@@ -154,6 +154,12 @@ int ovp_plane_measurement_compress_inplace(ovp_ctx *ctx, double *H_x, int cols, 
                                            int *rows_out);
 
 /* ---- UpdaterMSCKF::update from "features triangulated, plane CPs known" on (UpdaterMSCKF.cpp:407-828) --------------- */
+/* Track length: every feature of a batch has 2..39 measurements, or 2..37 when the batch runs a plane update (an in-state plane,
+ * a plane not in the state with >= 4 features, or ovp_plane_init).  Tracks of up to 32 run on one warp per feature; one longer
+ * track puts the whole batch on one CTA per feature, whose per-feature system must fit the CTA's shared memory.  A longer track
+ * is refused with OVP_ERR_CAPACITY before anything is launched, and the message names the limit.  Every other capacity check
+ * of the update (rows, columns, factorisation width) also runs before the first launch, so a refused batch leaves the state as
+ * it was. */
 typedef struct ovp_feature_batch {
   int F;                         /* number of features (feature_vec after triangulation, caller's order)               */
   const int *meas_offset;        /* F+1 prefix offsets into the measurement arrays                                      */
@@ -193,7 +199,8 @@ int ovp_plane_init(ovp_ctx *ctx, const ovp_feature_batch *batch, const ovp_updat
  * _features_SLAM_to_PLANE allows it) as state columns, chi2 gate against the marginal covariance, on failure WITH a plane
  * one retry without it (:547-609), then ONE EKF update with the stack of the accepted blocks (R = I).
  * planeid[f]: the feat2plane entry of the feature (0 = none).  feat_status[f]: 1 accepted (plane constraint included when the
- * feature had one), 3 accepted after dropping the plane constraint, 0 rejected (landmark flagged should_marg).  */
+ * feature had one), 3 accepted after dropping the plane constraint, 0 rejected (landmark flagged should_marg).
+ * Every landmark has 1..29 measurements; a longer track is refused with OVP_ERR_CAPACITY before anything is launched. */
 int ovp_slam_update(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
                     const int64_t *planeid, const ovp_updater_options *opt, int use_plane_constraint, int *feat_status,
                     double *feat_chi2);

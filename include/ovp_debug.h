@@ -2,7 +2,8 @@
  *
  * These entry points exist only in ov_plane_b200/lib/libovp_debug.so (the product sources compiled with -DOVP_DEBUG); the
  * product library libovp.so does not export them.  They let tools/microbench*.py measure single kernels and let
- * tests/test_gpu_cholfused.py unit-test chol_fused_kernel against NumPy on arbitrary matrices. */
+ * tests/test_gpu_cholfused.py / tests/test_gpu_gemm.py unit-test chol_fused_kernel and the DMMA GEMM against NumPy on arbitrary
+ * matrices. */
 #ifndef OVP_DEBUG_H
 #define OVP_DEBUG_H
 #include "ovp.h"
@@ -19,6 +20,15 @@ int ovp_debug_chol_fused(ovp_ctx *ctx, int n, int mrows, int iters, double *out,
  * when M is given, solve Y = M L^-T (mrows x npiv) and w = L^-1 z */
 int ovp_debug_chol_solve(ovp_ctx *ctx, const double *A, int n, int npiv, double tol, const double *M, int mrows, const double *z,
                          double *L_out, double *Y_out, double *w_out);
+/* one product C = alpha * A B + beta * C (+ diagonal) through the DMMA GEMM (tests/test_gpu_gemm.py).  Host matrices are column-major:
+ * A is a_rows x a_cols, logical A (M x K) = A, or A^T when a_trans; B is b_rows x b_cols, logical B (K x N) = B, or B^T when b_trans.
+ * akidx / bkidx (length K, or NULL) gather the contraction index of A / B.  C is ldc x N, updated in place.  diag_add (length
+ * min(M, N), or NULL) or diag_const is added on the diagonal.  tri: 0 full, 1 lower tiles, 2 lower mirrored; ktri as GemmProblem::ktri.
+ * flag >= 0 places a device flag of that value (0: the launch is a no-op).  tile: 32 or 64 forces the tile width, 0 lets the launcher
+ * choose.  info[0] = tile width launched, info[1] = SM count of the device. */
+int ovp_debug_gemm(ovp_ctx *ctx, int M, int N, int K, const double *A, int a_rows, int a_cols, int a_trans, const int *akidx, const double *B,
+                   int b_rows, int b_cols, int b_trans, const int *bkidx, double *C, int ldc, double alpha, double beta, const double *diag_add,
+                   double diag_const, int tri, int ktri, int flag, int tile, int *info);
 /* variants of the 16-column in-warp pivot chain (tools/microbench_potrf.py) */
 int ovp_debug_potrf_variants(ovp_ctx *ctx, int variant, int reps, double *out16);
 int ovp_debug_potrf_cond(ovp_ctx *ctx, int nthreads, int nchain, int smem_bytes, int reps, double *out16, int mode);

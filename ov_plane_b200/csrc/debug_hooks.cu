@@ -1,6 +1,6 @@
 // TEST / TUNING HOOKS — compiled only into libovp_debug.so (-DOVP_DEBUG), never into the product library libovp.so.
 // Declared in include/ovp_debug.h.  Used by tools/microbench*.py (latency and phase measurements of the fused Cholesky) and by
-// tests/test_gpu_cholfused.py (unit test of chol_fused_kernel against NumPy).
+// tests/test_gpu_cholfused.py and tests/test_gpu_gemm.py (unit tests of chol_fused_kernel and the DMMA GEMM against NumPy).
 #include "ovp_internal.h"
 using namespace ovp;
 
@@ -188,6 +188,57 @@ extern "C" int ovp_debug_chol_fused(ovp_ctx *h, int n, int mrows, int iters, dou
     return fail(c, OVP_ERR_NOT_POSITIVE_DEFINITE, "debug_chol_fused: test matrix not positive definite");
   }
   return OVP_OK;
+}
+
+// Test hook for the DMMA GEMM (tests/test_gpu_gemm.py): one GemmProblem on host operands through launch_gemm, tile width forced or
+// automatic.  Not part of the ABI in include/ovp.h.
+extern "C" int ovp_debug_gemm(ovp_ctx *h, int M, int N, int K, const double *A, int a_rows, int a_cols, int a_trans, const int *akidx,
+                              const double *B, int b_rows, int b_cols, int b_trans, const int *bkidx, double *C, int ldc, double alpha,
+                              double beta, const double *diag_add, double diag_const, int tri, int ktri, int flag, int tile, int *info) {
+  Ctx *c = ovp::enter(h);
+  if (M < 0 || N < 0 || K < 0 || ldc < M || a_rows < 1 || a_cols < 1 || b_rows < 1 || b_cols < 1 || (tile != 0 && tile != 32 && tile != 64))
+    return fail(c, OVP_ERR_BAD_ARGS, "debug_gemm: bad sizes");
+  const size_t na = (size_t)a_rows * a_cols, nb = (size_t)b_rows * b_cols, nc = (size_t)ldc * std::max(N, 1);
+  const size_t nd = (size_t)std::max(1, std::min(M, N));
+  const size_t bytes = (na + nb + nc + nd) * sizeof(double) + 2 * ((size_t)K + 1) * sizeof(int) + 16;
+  char *buf = nullptr;
+  OVP_CUDA(cudaMalloc(&buf, bytes));
+  double *dA = (double *)buf, *dB = dA + na, *dC = dB + nb, *dD = dC + nc;
+  int *dak = (int *)(dD + nd), *dbk = dak + K + 1, *dflag = dbk + K + 1;
+  int st = OVP_OK;
+  auto run = [&]() -> int {
+    OVP_CUDA(cudaMemcpyAsync(dA, A, na * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    OVP_CUDA(cudaMemcpyAsync(dB, B, nb * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    OVP_CUDA(cudaMemcpyAsync(dC, C, nc * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    if (diag_add)
+      OVP_CUDA(cudaMemcpyAsync(dD, diag_add, std::min(M, N) * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    if (akidx && K)
+      OVP_CUDA(cudaMemcpyAsync(dak, akidx, K * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    if (bkidx && K)
+      OVP_CUDA(cudaMemcpyAsync(dbk, bkidx, K * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    OVP_CUDA(cudaMemcpyAsync(dflag, &flag, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    // logical A (M x K): gathers index the physical column (plain) or row (transposed); logical B (K x N): the physical row or column
+    MatView va = a_trans ? mv(dA, a_rows, 1, akidx ? dak : nullptr, nullptr) : mv(dA, a_rows, 0, nullptr, akidx ? dak : nullptr);
+    MatView vb = b_trans ? mv(dB, b_rows, 1, nullptr, bkidx ? dbk : nullptr) : mv(dB, b_rows, 0, bkidx ? dbk : nullptr, nullptr);
+    GemmProblem p = make_problem(M, N, K, va, vb, dC, ldc, alpha, beta);
+    p.diag_add = diag_add ? dD : nullptr;
+    p.diag_const = diag_const;
+    p.tri = tri;
+    p.ktri = ktri;
+    GemmBatch b;
+    b.n = 1;
+    b.p[0] = p;
+    b.flag = flag >= 0 ? dflag : nullptr;
+    info[0] = launch_gemm(c, b, tile);
+    info[1] = c->num_sms;
+    OVP_CUDA(cudaGetLastError());
+    OVP_CUDA(cudaMemcpyAsync(C, dC, nc * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaStreamSynchronize(c->stream));
+    return OVP_OK;
+  };
+  st = run();
+  cudaFree(buf);
+  return st;
 }
 
 // Test hook for the fused Cholesky (tests/test_gpu_cholfused.py): factor a host matrix (lower triangle of A, n x n, column-major)

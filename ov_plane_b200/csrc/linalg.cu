@@ -31,7 +31,7 @@ template <int TILE> static void launch_gemm_tile(Ctx *c, const GemmBatch &b, dim
   else
     gemm_f64_kernel<TILE, false, false><<<grid, 128, 0, c->stream>>>(b);
 }
-void launch_gemm(Ctx *c, const GemmBatch &b) {
+int launch_gemm(Ctx *c, const GemmBatch &b, int tile) {
   int tm = 0, tn = 0;
   long long tiles64 = 0;
   double work = 0;
@@ -43,9 +43,11 @@ void launch_gemm(Ctx *c, const GemmBatch &b) {
     work += (b.p[i].tri == TRI_FULL ? 2.0 : 1.0) * (double)b.p[i].M * b.p[i].N * b.p[i].K;
   }
   if (tm == 0 || tn == 0 || b.n == 0)
-    return;
+    return 0;
+  if (tile != 32 && tile != 64) // below one wave of 64-wide tiles, 32-wide ones give more CTAs to hide the k-loop latency
+    tile = tiles64 >= c->num_sms ? 64 : 32;
   prof_begin(c, PROF_GEMM, work);
-  if (tiles64 >= c->num_sms) { // below one wave of 64-wide tiles, 32-wide ones give more CTAs to hide the k-loop latency
+  if (tile == 64) {
     launch_gemm_tile<64>(c, b, dim3(tn, tm, b.n));
   } else { // fewer 64-tiles than SMs: 32-tiles quadruple the CTA count and quarter the per-CTA tensor work
     int tm32 = 0, tn32 = 0;
@@ -57,6 +59,7 @@ void launch_gemm(Ctx *c, const GemmBatch &b) {
   }
   c->launches++;
   prof_end(c);
+  return tile;
 }
 
 static cudaEvent_t prof_event(Ctx *c) {

@@ -164,7 +164,14 @@ int fail(Ctx *c, int status, const char *fmt, ...);
 // ---- linalg.cu ---------------------------------------------------------------------------------------------------
 int chol_fused(Ctx *c, double *A, int ld, int n, int npiv, double tol, const double *M, int ldm, int mrows, const double *z, int zstride,
                double *Y, int ldy, double *w, double gate_thresh, double *chi2, int *gate_flag, long long *dbg = nullptr);
-void launch_gemm(Ctx *c, const GemmBatch &b);
+// every tile CTA of one chol_fused launch must be co-resident: the tile CTAs a factorisation of the leading npiv columns of an n x n
+// system needs, how many the device holds, and the widest full factorisation (a multiple of 64) that fits
+int chol_fused_tiles(int n, int npiv);
+int chol_fused_capacity(Ctx *c, int *max_tiles);
+int chol_fused_width(Ctx *c, int *width);
+// tile = 0: 64-wide tiles when the batch has at least one 64-tile per SM, else 32-wide; 32 / 64 force the width (test hook).
+// Returns the tile width launched (0: nothing to do).
+int launch_gemm(Ctx *c, const GemmBatch &b, int tile = 0);
 void launch_gemm1(Ctx *c, const GemmProblem &p, const int *flag = nullptr);
 // In-place blocked Cholesky of the leading `npiv` pivots of the symmetric (lower-stored) matrix A (size n x n, ld):
 int chol_partial(Ctx *c, double *A, int ld, int n, int npiv, double tol); // one launch of chol_fused
