@@ -1,9 +1,9 @@
 /* TEST / TUNING HOOKS of the H100-native ov_plane hot path — NOT part of the drop-in ABI (include/ovp.h).
  *
  * These entry points exist only in ov_plane_b200/lib/libovp_debug.so (the product sources compiled with -DOVP_DEBUG); the
- * product library libovp.so does not export them.  They let tools/microbench*.py measure single kernels and let
+ * product library libovp.so does not export them.  They let tools/microbench_chol.py time the fused Cholesky, let
  * tests/test_gpu_cholfused.py / tests/test_gpu_gemm.py unit-test chol_fused_kernel and the DMMA GEMM against NumPy on arbitrary
- * matrices. */
+ * matrices, and let tests/test_gpu_numerics.py run one batch through both MSCKF feature paths. */
 #ifndef OVP_DEBUG_H
 #define OVP_DEBUG_H
 #include "ovp.h"
@@ -11,8 +11,6 @@
 extern "C" {
 #endif
 
-/* dependent-chain latencies (cycles per operation, one warp) of DFMA, rsqrt, 1/x, sqrt, shuffles, shared-memory loads, DMMA */
-int ovp_debug_fp64_latency(ovp_ctx *ctx, double *out8);
 /* fused Cholesky on a synthetic SPD n x n system (+ mrows x n right-hand side): out[0] = us per (fill + factor), out[1] = us per
  * fill, out[2..] = per-CTA globaltimer stamps of the last run */
 int ovp_debug_chol_fused(ovp_ctx *ctx, int n, int mrows, int iters, double *out, int out_cap);
@@ -29,9 +27,9 @@ int ovp_debug_chol_solve(ovp_ctx *ctx, const double *A, int n, int npiv, double 
 int ovp_debug_gemm(ovp_ctx *ctx, int M, int N, int K, const double *A, int a_rows, int a_cols, int a_trans, const int *akidx, const double *B,
                    int b_rows, int b_cols, int b_trans, const int *bkidx, double *C, int ldc, double alpha, double beta, const double *diag_add,
                    double diag_const, int tri, int ktri, int flag, int tile, int *info);
-/* variants of the 16-column in-warp pivot chain (tools/microbench_potrf.py) */
-int ovp_debug_potrf_variants(ovp_ctx *ctx, int variant, int reps, double *out16);
-int ovp_debug_potrf_cond(ovp_ctx *ctx, int nthreads, int nchain, int smem_bytes, int reps, double *out16, int mode);
+/* on != 0: every later ovp_msckf_update of this context builds its point and plane systems with the one-block-per-feature kernel and
+ * the dense stacked Gram matrix, also when all its tracks fit the warp-per-feature path (at most 32 measurements) */
+int ovp_debug_force_dense_features(ovp_ctx *ctx, int on);
 
 #ifdef __cplusplus
 }

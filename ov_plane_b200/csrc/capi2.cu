@@ -533,22 +533,20 @@ namespace ovp {
 static int stage_feature_jacobian(Ctx *c, int m, const int *clone_handles, const float *uv, const double *p_FinG, const double *p_FinG_fej,
                                   bool has_plane, int plane_handle, const double *cp, const double *cp_fej, double sigma_px, double sigma_c,
                                   int *rows_out, int *hfc_out, int *hxc_out, int extra_hx_cols = 0) {
-  if (m < 1 || m > 64)
+  if (m > 64) // a size argument, not a track a feature kernel holds
     return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full: m=%d not in 1..64", m);
-  for (int i = 0; i < m; i++) {
-    if (!valid_handle(c, clone_handles[i]) || c->vars[clone_handles[i]].kind != OVP_KIND_POSE)
-      return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full: handle %d is not a clone", clone_handles[i]);
-    for (int j = 0; j < i; j++)
-      if (clone_handles[j] == clone_handles[i])
-        return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full: duplicate clone (mono camera assumed)");
-  }
+  const int off[2] = {0, m};
+  int mmax;
+  int st = check_tracks(c, 1, off, clone_handles, 1, 0, false, &mmax); // a live pose, with or without covariance columns
+  if (st)
+    return st;
   const bool in_state = has_plane && plane_handle >= 0;
   const int ncal = (c->opt.do_calib_camera_pose ? 6 : 0) + (c->opt.do_calib_camera_intrinsics ? 8 : 0);
   const int rows = has_plane ? 3 * m : 2 * m;
   const int hfc = 3 + ((has_plane && !in_state) ? 3 : 0);
   const int hxc = ncal + 6 * m + (in_state ? 3 : 0) + extra_hx_cols; // extra: zero columns appended for an anchor clone (anchors.cu)
   size_t e = (size_t)rows * (hfc + hxc + 1) + 256;
-  int st = ensure_stage(c, e);
+  st = ensure_stage(c, e);
   if (st)
     return st;
   OVP_CUDA(cudaMemsetAsync(c->d_stage, 0, e * sizeof(double), c->stream));
@@ -792,22 +790,14 @@ int ovp_msckf_update(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updat
 }
 
 static int shard_cols(Ctx *c, const int *all_clone_handles, int n_clones, std::vector<int> &cols) {
-  std::vector<std::pair<int, int>> blocks;
-  if (c->opt.do_calib_camera_pose)
-    blocks.push_back({c->vars[c->h_calib].id, 6});
-  if (c->opt.do_calib_camera_intrinsics)
-    blocks.push_back({c->vars[c->h_intr].id, 8});
+  std::vector<std::pair<int, int>> clones;
   for (int i = 0; i < n_clones; i++) {
     int hh = all_clone_handles[i];
-    if (!valid_handle(c, hh) || c->vars[hh].kind != OVP_KIND_POSE || c->vars[hh].id < 0)
+    if (!is_clone(c, hh, true))
       return fail(c, OVP_ERR_BAD_ARGS, "shard: handle %d is not a clone in the state", hh);
-    blocks.push_back({c->vars[hh].id, 6});
+    clones.push_back({c->vars[hh].id, 6});
   }
-  std::sort(blocks.begin(), blocks.end());
-  cols.clear();
-  for (auto &b : blocks)
-    for (int j = 0; j < b.second; j++)
-      cols.push_back(b.first + j);
+  cols = compact_cols(c, std::move(clones));
   return OVP_OK;
 }
 int ovp_msckf_shard_columns(ovp_ctx *h, const int *all_clone_handles, int n_clones, int *n_cols) {

@@ -1,121 +1,9 @@
 // TEST / TUNING HOOKS — compiled only into libovp_debug.so (-DOVP_DEBUG), never into the product library libovp.so.
-// Declared in include/ovp_debug.h.  Used by tools/microbench*.py (latency and phase measurements of the fused Cholesky) and by
-// tests/test_gpu_cholfused.py and tests/test_gpu_gemm.py (unit tests of chol_fused_kernel and the DMMA GEMM against NumPy).
+// Declared in include/ovp_debug.h.  Used by tools/microbench_chol.py (phase timeline of the fused Cholesky), by
+// tests/test_gpu_cholfused.py and tests/test_gpu_gemm.py (unit tests of chol_fused_kernel and the DMMA GEMM against NumPy) and by
+// tests/test_gpu_numerics.py (the block-sparse feature path against the dense stack on the same batch).
 #include "ovp_internal.h"
 using namespace ovp;
-
-// ---- micro-benchmarks of single kernels (tools/microbench.py) ------------------------------------------------------------
-namespace ovp {
-// dependent-chain latencies of fp64 operations on this GPU (cycles per op), one warp
-__global__ void fp64_latency_kernel(double *out, double seed) {
-  double x = seed + threadIdx.x * 1e-9;
-  long long t0, t1;
-  const int N = 256;
-  t0 = clock64();
-#pragma unroll 16
-  for (int i = 0; i < N; i++)
-    x = fma(x, 1.0000001, 1e-9);
-  t1 = clock64();
-  if (threadIdx.x == 0)
-    out[0] = (double)(t1 - t0) / N;
-  double y = x;
-  t0 = clock64();
-#pragma unroll 4
-  for (int i = 0; i < N; i++)
-    y = rsqrt(y) + 1.5;
-  t1 = clock64();
-  if (threadIdx.x == 0)
-    out[1] = (double)(t1 - t0) / N;
-  double z = y;
-  t0 = clock64();
-#pragma unroll 4
-  for (int i = 0; i < N; i++)
-    z = 1.0 / z + 1.5;
-  t1 = clock64();
-  if (threadIdx.x == 0)
-    out[2] = (double)(t1 - t0) / N;
-  double w = z;
-  t0 = clock64();
-#pragma unroll 4
-  for (int i = 0; i < N; i++)
-    w = sqrt(w) + 1.5;
-  t1 = clock64();
-  if (threadIdx.x == 0)
-    out[3] = (double)(t1 - t0) / N;
-  // shuffle of a double, dependent
-  double s = w;
-  t0 = clock64();
-#pragma unroll 16
-  for (int i = 0; i < N; i++)
-    s = __shfl_sync(0xffffffffu, s, (threadIdx.x + 1) & 31);
-  t1 = clock64();
-  if (threadIdx.x == 0)
-    out[4] = (double)(t1 - t0) / N;
-  // shared-memory dependent load chain
-  __shared__ double sh[64];
-  sh[threadIdx.x] = (double)((threadIdx.x * 7 + 3) & 31);
-  __syncwarp();
-  int idx = threadIdx.x;
-  t0 = clock64();
-#pragma unroll 16
-  for (int i = 0; i < N; i++)
-    idx = (int)sh[idx];
-  t1 = clock64();
-  if (threadIdx.x == 0)
-    out[5] = (double)(t1 - t0) / N;
-  // float rsqrt + 2 Newton steps in fp64 (candidate fast path)
-  double q = s + 2.0 + idx;
-  t0 = clock64();
-#pragma unroll 4
-  for (int i = 0; i < N; i++) {
-    double y0 = (double)rsqrtf((float)q);
-    y0 = y0 * fma(-0.5 * q * y0, y0, 1.5);
-    y0 = y0 * fma(-0.5 * q * y0, y0, 1.5);
-    q = y0 + 1.5;
-  }
-  t1 = clock64();
-  if (threadIdx.x == 0) {
-    out[6] = (double)(t1 - t0) / N;
-    out[7] = x + y + z + w + s + q;
-  }
-  // DMMA m8n8k4: dependent chain (latency) and 8 independent accumulators (issue rate of one warp)
-  double c0 = 0.0, c1 = 0.0, aa = 1.0 + 1e-9 * threadIdx.x, bb = 1.0 - 1e-9 * threadIdx.x;
-  t0 = clock64();
-#pragma unroll 16
-  for (int i = 0; i < N; i++)
-    dmma_m8n8k4(c0, c1, aa, bb);
-  t1 = clock64();
-  if (threadIdx.x == 0)
-    out[8] = (double)(t1 - t0) / N;
-  double e[8][2];
-#pragma unroll
-  for (int k = 0; k < 8; k++)
-    e[k][0] = e[k][1] = 0.0;
-  t0 = clock64();
-#pragma unroll 4
-  for (int i = 0; i < N / 8; i++)
-#pragma unroll
-    for (int k = 0; k < 8; k++)
-      dmma_m8n8k4(e[k][0], e[k][1], aa, bb);
-  t1 = clock64();
-  double sum = c0 + c1;
-#pragma unroll
-  for (int k = 0; k < 8; k++)
-    sum += e[k][0] + e[k][1];
-  if (threadIdx.x == 0) {
-    out[9] = (double)(t1 - t0) / N;
-    out[10] = sum;
-  }
-}
-} // namespace ovp
-extern "C" int ovp_debug_fp64_latency(ovp_ctx *h, double *out8) {
-  Ctx *c = ovp::enter(h);
-  fp64_latency_kernel<<<1, 32, 0, c->stream>>>(c->dscal + 160, 1.2345);
-  OVP_CUDA(cudaStreamSynchronize(c->stream));
-  OVP_CUDA(cudaMemcpy(out8, c->dscal + 160, 10 * sizeof(double), cudaMemcpyDeviceToHost));
-  return OVP_OK;
-}
-
 
 namespace ovp {
 __global__ void spd_fill_kernel(double *A, int ld, int n) {
@@ -276,5 +164,12 @@ extern "C" int ovp_debug_chol_solve(ovp_ctx *h, const double *A, int n, int npiv
     cudaMemset(c->dflags + 1, 0, sizeof(int));
     return fail(c, OVP_ERR_NOT_POSITIVE_DEFINITE, "debug_chol_solve: matrix not positive definite (strict mode)");
   }
+  return OVP_OK;
+}
+
+// Test hook (tests/test_gpu_numerics.py): on != 0 sends every later MSCKF batch of this context through the one-block-per-feature kernel
+// and the dense stacked system, whatever its longest track; the plan signature includes the setting.  Not part of the ABI in include/ovp.h.
+extern "C" int ovp_debug_force_dense_features(ovp_ctx *h, int on) {
+  h->c.force_dense_features = on != 0;
   return OVP_OK;
 }

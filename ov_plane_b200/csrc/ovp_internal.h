@@ -50,6 +50,7 @@ struct Ctx {
   int64_t launches = 0;
   bool use_graphs = true;    // replay the static launch sequence of a prepared batch as a CUDA graph
   double gram_tol = 1e-11;   // zero-pivot rule of the Gram Cholesky, relative to the column's original diagonal (ovp_set_rank_tolerance)
+  bool force_dense_features = false; // MSCKF batches take the one-block-per-feature kernel and the dense stack (ovp_debug_force_dense_features)
 
   // --- State mirror -------------------------------------------------------------------------------------------
   int Nmax = 0, ldP = 0, N = 0;

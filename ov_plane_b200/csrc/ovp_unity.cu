@@ -9,5 +9,4 @@
 #include "anchors.cu"
 #ifdef OVP_DEBUG // libovp_debug.so only: micro-benchmarks and kernel-level test hooks (include/ovp_debug.h)
 #include "debug_hooks.cu"
-#include "debug_potrf.cu"
 #endif

@@ -28,19 +28,24 @@ def test_library_exports_every_declared_symbol():
     assert not missing, missing
 
 
-def test_product_library_exports_only_the_declared_abi():
-    """libovp.so exports exactly the symbols of include/ovp.h: no test / tuning hooks (those live in libovp_debug.so and are
-    declared in include/ovp_debug.h)."""
+def _exported(path, prefix):
     import subprocess
+    out = subprocess.check_output(["nm", "-D", "--defined-only", path]).decode()
+    return sorted(set(re.findall(r"\b T (%s[a-z0-9_]+)$" % prefix, out, flags=re.M)))
+
+
+def test_libraries_export_exactly_the_declared_symbols():
+    """libovp.so exports exactly the symbols of include/ovp.h: no test / tuning hooks (those live in libovp_debug.so and are
+    declared in include/ovp_debug.h); libovp_debug.so exports exactly the hooks include/ovp_debug.h declares, and the whole ABI."""
     from ov_plane_b200 import api
-    out = subprocess.check_output(["nm", "-D", "--defined-only", api.LIB_PATH]).decode()
-    exported = sorted(set(re.findall(r"\b T (ovp_[a-z0-9_]+)$", out, flags=re.M)))
+    exported = _exported(api.LIB_PATH, "ovp_")
     assert exported == declared_symbols(), sorted(set(exported) ^ set(declared_symbols()))
     txt = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "ovp_debug.h")).read(), flags=re.S)
     hooks = sorted(set(re.findall(r"\b(ovp_debug_[a-z0-9_]+)\s*\(", txt)))
-    assert len(hooks) >= 5
+    assert hooks
+    dbg_hooks = _exported(api.DEBUG_LIB_PATH, "ovp_debug_")
+    assert dbg_hooks == hooks, sorted(set(dbg_hooks) ^ set(hooks))
     dbg = ctypes.CDLL(api.DEBUG_LIB_PATH)
-    assert not [h for h in hooks if not hasattr(dbg, h)]
     assert not [s for s in declared_symbols() if not hasattr(dbg, s)]
 
 

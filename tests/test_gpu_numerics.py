@@ -170,22 +170,19 @@ def test_handle_table_stays_bounded_over_a_long_run(chi2_table):
 @pytest.mark.parametrize("name", ["cfg1_euroc_n96", "small_planes", "cfg3_n512_f600_p8"])
 def test_block_sparse_gram_equals_dense_stacked_path(name, chi2_table):
     """The warp-per-feature path (G = D - Y^T Y, never materialising the stacked Jacobian, msckf_warp.inc) against the dense stacked
-    path (feature_kernel + SYRK over all projected rows; OVP_DENSE_STACK=1): same gates, chi2 and posterior."""
-    import os
+    path (feature_kernel + SYRK over all projected rows; the ovp_debug_force_dense_features hook of libovp_debug.so): same gates, chi2
+    and posterior."""
     S = synth.make_scenario(name, seed=0)
     out = {}
-    for mode in ("0", "1"):
-        os.environ["OVP_DENSE_STACK"] = mode
-        try:
-            ctx = api.Context(S.options, device=0, max_state=max(128, S.N + 64), max_meas_rows=60000)
-            ctx.set_chi2_table(chi2_table)
-            ch = synth.load_scenario_into(ctx, S)
-            r = ctx.msckf_update(synth.feature_batch(S, ch), 1.0, 1.0)
-            out[mode] = (r, ctx.cov(), ctx.launch_count())
-            ctx.close()
-        finally:
-            os.environ.pop("OVP_DENSE_STACK", None)
-    (r0, P0, l0), (r1, P1, l1) = out["0"], out["1"]
+    for dense in (0, 1):
+        ctx = api.Context(S.options, device=0, max_state=max(128, S.N + 64), max_meas_rows=60000, debug=True)
+        ctx._ck(ctx.lib.ovp_debug_force_dense_features(ctx.h, dense))
+        ctx.set_chi2_table(chi2_table)
+        ch = synth.load_scenario_into(ctx, S)
+        r = ctx.msckf_update(synth.feature_batch(S, ch), 1.0, 1.0)
+        out[dense] = (r, ctx.cov(), ctx.launch_count())
+        ctx.close()
+    (r0, P0, l0), (r1, P1, l1) = out[0], out[1]
     assert np.array_equal(r0["feat_status"], r1["feat_status"]) and np.array_equal(r0["plane_status"], r1["plane_status"])
     m = (r0["feat_status"] == 0) | (r0["feat_status"] == 1)
     e_chi = np.abs(r0["feat_chi2"][m] / r1["feat_chi2"][m] - 1).max() if m.any() else 0.0
