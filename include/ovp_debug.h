@@ -2,7 +2,7 @@
  *
  * These entry points exist only in ov_plane_b200/lib/libovp_debug.so (the product sources compiled with -DOVP_DEBUG); the
  * product library libovp.so does not export them.  They let tools/microbench_chol.py time the fused Cholesky, let
- * tests/test_gpu_cholfused.py / tests/test_gpu_gemm.py unit-test chol_fused_kernel and the DMMA GEMM against NumPy on arbitrary
+ * tests/test_gpu_cholfused.py / tests/test_gpu_gemm.py / tests/test_gpu_gemm_split.py unit-test chol_fused_kernel and the DMMA GEMM against NumPy on arbitrary
  * matrices, and let tests/test_gpu_numerics.py run one batch through both MSCKF feature paths. */
 #ifndef OVP_DEBUG_H
 #define OVP_DEBUG_H
@@ -27,6 +27,10 @@ int ovp_debug_chol_solve(ovp_ctx *ctx, const double *A, int n, int npiv, double 
 int ovp_debug_gemm(ovp_ctx *ctx, int M, int N, int K, const double *A, int a_rows, int a_cols, int a_trans, const int *akidx, const double *B,
                    int b_rows, int b_cols, int b_trans, const int *bkidx, double *C, int ldc, double alpha, double beta, const double *diag_add,
                    double diag_const, int tri, int ktri, int flag, int tile, int *info);
+/* the k split the DMMA GEMM takes for one product of these sizes (tests/test_gpu_gemm_split.py): info[0] = tile width (tile 32 / 64 forces
+ * it, 0 lets the launcher choose, as in ovp_debug_gemm), info[1] = chunk count, info[2] = chunk length kc.  Chunk c covers
+ * [c kc, min(K, (c + 1) kc)); one chunk is the unsplit k walk. */
+int ovp_debug_gemm_split(ovp_ctx *ctx, int M, int N, int K, int tri, int ktri, int tile, int *info);
 /* on != 0: every later ovp_msckf_update of this context builds its point and plane systems with the one-block-per-feature kernel and
  * the dense stacked Gram matrix, also when all its tracks fit the warp-per-feature path (at most 32 measurements) */
 int ovp_debug_force_dense_features(ovp_ctx *ctx, int on);

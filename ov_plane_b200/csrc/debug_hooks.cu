@@ -129,6 +129,23 @@ extern "C" int ovp_debug_gemm(ovp_ctx *h, int M, int N, int K, const double *A, 
   return st;
 }
 
+// Test hook for the DMMA GEMM's k split (tests/test_gpu_gemm_split.py): the tile width and the chunks launch_gemm takes for one product of
+// these sizes.  Not part of the ABI in include/ovp.h.
+extern "C" int ovp_debug_gemm_split(ovp_ctx *h, int M, int N, int K, int tri, int ktri, int tile, int *info) {
+  Ctx *c = ovp::enter(h);
+  if (M < 0 || N < 0 || K < 0 || (tile != 0 && tile != 32 && tile != 64))
+    return fail(c, OVP_ERR_BAD_ARGS, "debug_gemm_split: bad sizes");
+  GemmProblem p = make_problem(M, N, K, mv(nullptr, 1), mv(nullptr, 1), nullptr, std::max(M, 1));
+  p.tri = tri;
+  p.ktri = ktri;
+  GemmBatch b;
+  b.n = 1;
+  b.p[0] = p;
+  b.flag = nullptr;
+  info[0] = gemm_plan(c, b, tile, &info[1], &info[2]);
+  return OVP_OK;
+}
+
 // Test hook for the fused Cholesky (tests/test_gpu_cholfused.py): factor a host matrix (lower triangle of A, n x n, column-major)
 // over its leading npiv columns with pivot tolerance tol and, when M is given, solve Y = M L^-T (mrows x npiv) and w = L^-1 z.
 // Not part of the ABI in include/ovp.h.

@@ -312,6 +312,7 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
   {
     GemmProblem p = make_problem(N, N, rr, mv(c->dY, c->Nmax), mv(c->dY, c->Nmax, 1), c->dP, c->ldP, -1.0, 1.0);
     p.tri = TRI_LOWER_MIRROR;
+    p.nosplit = 1; // on the side stream it hides behind the next update's launches; unsplit it takes fewer SMs from them (DESIGN.md §9)
     launch_gemm1(c, p, flag);
   }
   diag_check_kernel<<<(N + 255) / 256, 256, 0, c->stream>>>(c->dP, c->ldP, N, c->dflags, flag);

@@ -20,42 +20,91 @@ int fail(Ctx *c, int status, const char *fmt, ...) {
   return status;
 }
 
-template <int TILE> static void launch_gemm_tile(Ctx *c, const GemmBatch &b, dim3 grid) {
+template <int TILE, bool GA, bool GB> static void launch_gemm_kernel(Ctx *c, const GemmBatch &b, dim3 grid, int nchunk, int kc) {
+  const size_t smem = gemm_smem_bytes<TILE>(GA, GB, kc);
+  if (smem > 48 * 1024) // the 64-wide tile's stages, or a long gather-index slice: opt in to more than the default 48 KB
+    cudaFuncSetAttribute(gemm_f64_kernel<TILE, GA, GB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = dim3(128);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = c->stream;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 1;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = nchunk; // the chunks of one output tile
+  cfg.attrs = &attr;
+  cfg.numAttrs = nchunk > 1 ? 1 : 0;
+  cudaLaunchKernelEx(&cfg, gemm_f64_kernel<TILE, GA, GB>, b, nchunk, kc);
+}
+template <int TILE> static void launch_gemm_tile(Ctx *c, const GemmBatch &b, dim3 grid, int nchunk, int kc) {
   const bool ga = b.p[0].A.kidx != nullptr, gb = b.p[0].B.kidx != nullptr;
   if (ga && gb)
-    gemm_f64_kernel<TILE, true, true><<<grid, 128, 0, c->stream>>>(b);
+    launch_gemm_kernel<TILE, true, true>(c, b, grid, nchunk, kc);
   else if (ga)
-    gemm_f64_kernel<TILE, true, false><<<grid, 128, 0, c->stream>>>(b);
+    launch_gemm_kernel<TILE, true, false>(c, b, grid, nchunk, kc);
   else if (gb)
-    gemm_f64_kernel<TILE, false, true><<<grid, 128, 0, c->stream>>>(b);
+    launch_gemm_kernel<TILE, false, true>(c, b, grid, nchunk, kc);
   else
-    gemm_f64_kernel<TILE, false, false><<<grid, 128, 0, c->stream>>>(b);
+    launch_gemm_kernel<TILE, false, false>(c, b, grid, nchunk, kc);
 }
-int launch_gemm(Ctx *c, const GemmBatch &b, int tile) {
-  int tm = 0, tn = 0;
-  long long tiles64 = 0;
-  double work = 0;
+
+// Shortest k chunk of a split launch: 8 k-steps of 16.  On an H100, chunks of 64 (up to 8 per tile) made the benchmark step slower than
+// chunks of 128 (up to 4): more CTAs, half of them dead under ktri, and twice the reduction traffic for the same k walk (DESIGN.md §9).
+static constexpr int kGemmMinChunk = 128;
+
+int gemm_plan(const Ctx *c, const GemmBatch &b, int tile, int *nchunk, int *kc) {
+  long long tiles64 = 0, tiles = 0;
+  int K = 0;
+  bool nosplit = false;
   for (int i = 0; i < b.n; i++) {
     int a = (b.p[i].M + 63) / 64, bb = (b.p[i].N + 63) / 64;
-    tm = std::max(tm, a);
-    tn = std::max(tn, bb);
     tiles64 += (b.p[i].tri == TRI_FULL) ? (long long)a * bb : (long long)a * (a + 1) / 2;
+    K = std::max(K, b.p[i].K);
+    nosplit |= b.p[i].nosplit != 0;
+  }
+  if (tile != 32 && tile != 64) // below one wave of 64-wide tiles, 32-wide ones give more CTAs to hide the k-loop latency
+    tile = tiles64 >= c->num_sms ? 64 : 32;
+  for (int i = 0; i < b.n; i++) {
+    int a = (b.p[i].M + tile - 1) / tile, bb = (b.p[i].N + tile - 1) / tile;
+    tiles += (b.p[i].tri == TRI_FULL) ? (long long)a * bb : (long long)a * (a + 1) / 2;
+  }
+  // Split k when the tiles alone are less than two waves and K is longer than one chunk: up to OVP_GSPLIT_MAX chunks of at least
+  // kGemmMinChunk, kc rounded up to the k-step.  Only the shapes, the tile width and the SM count enter, so a product always sums
+  // in the same order (auto and forced tile widths included).
+  int n = 1;
+  if (!nosplit && tiles < 2LL * c->num_sms && K > kGemmMinChunk)
+    n = std::min(OVP_GSPLIT_MAX, (K + kGemmMinChunk - 1) / kGemmMinChunk);
+  int len = ((K + n - 1) / n + OVP_GK - 1) / OVP_GK * OVP_GK;
+  len = std::max(len, OVP_GK);
+  *kc = len;
+  *nchunk = std::max(1, (K + len - 1) / len);
+  return tile;
+}
+
+int launch_gemm(Ctx *c, const GemmBatch &b, int tile) {
+  int tm = 0, tn = 0;
+  double work = 0;
+  for (int i = 0; i < b.n; i++) {
+    tm = std::max(tm, (b.p[i].M + 63) / 64);
+    tn = std::max(tn, (b.p[i].N + 63) / 64);
     work += (b.p[i].tri == TRI_FULL ? 2.0 : 1.0) * (double)b.p[i].M * b.p[i].N * b.p[i].K;
   }
   if (tm == 0 || tn == 0 || b.n == 0)
     return 0;
-  if (tile != 32 && tile != 64) // below one wave of 64-wide tiles, 32-wide ones give more CTAs to hide the k-loop latency
-    tile = tiles64 >= c->num_sms ? 64 : 32;
+  int nchunk = 1, kc = OVP_GK;
+  tile = gemm_plan(c, b, tile, &nchunk, &kc);
   prof_begin(c, PROF_GEMM, work);
   if (tile == 64) {
-    launch_gemm_tile<64>(c, b, dim3(tn, tm, b.n));
+    launch_gemm_tile<64>(c, b, dim3(tn, tm, b.n * nchunk), nchunk, kc);
   } else { // fewer 64-tiles than SMs: 32-tiles quadruple the CTA count and quarter the per-CTA tensor work
     int tm32 = 0, tn32 = 0;
     for (int i = 0; i < b.n; i++) {
       tm32 = std::max(tm32, (b.p[i].M + 31) / 32);
       tn32 = std::max(tn32, (b.p[i].N + 31) / 32);
     }
-    launch_gemm_tile<32>(c, b, dim3(tn32, tm32, b.n));
+    launch_gemm_tile<32>(c, b, dim3(tn32, tm32, b.n * nchunk), nchunk, kc);
   }
   c->launches++;
   prof_end(c);

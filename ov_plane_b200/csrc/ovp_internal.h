@@ -173,6 +173,8 @@ int chol_fused_width(Ctx *c, int *width);
 // tile = 0: 64-wide tiles when the batch has at least one 64-tile per SM, else 32-wide; 32 / 64 force the width (test hook).
 // Returns the tile width launched (0: nothing to do).
 int launch_gemm(Ctx *c, const GemmBatch &b, int tile = 0);
+// the tile width (returned) and the k split (chunk count, chunk length) launch_gemm uses for b; tile 32 / 64 forces the width
+int gemm_plan(const Ctx *c, const GemmBatch &b, int tile, int *nchunk, int *kc);
 void launch_gemm1(Ctx *c, const GemmProblem &p, const int *flag = nullptr);
 // In-place blocked Cholesky of the leading `npiv` pivots of the symmetric (lower-stored) matrix A (size n x n, ld):
 int chol_partial(Ctx *c, double *A, int ld, int n, int npiv, double tol); // one launch of chol_fused
