@@ -3,7 +3,8 @@
  * These entry points exist only in ov_plane_b200/lib/libovp_debug.so (the product sources compiled with -DOVP_DEBUG); the
  * product library libovp.so does not export them.  They let tools/microbench_chol.py time the fused Cholesky, let
  * tests/test_gpu_cholfused.py / tests/test_gpu_gemm.py / tests/test_gpu_gemm_split.py unit-test chol_fused_kernel and the DMMA GEMM against NumPy on arbitrary
- * matrices, and let tests/test_gpu_numerics.py run one batch through both MSCKF feature paths. */
+ * matrices, let tests/test_gpu_numerics.py run one batch through both MSCKF feature paths, and let tests/test_gpu_fused_products.py check the
+ * update products formed inside the Gram factorisation and run the update both with and without them. */
 #ifndef OVP_DEBUG_H
 #define OVP_DEBUG_H
 #include "ovp.h"
@@ -34,6 +35,15 @@ int ovp_debug_gemm_split(ovp_ctx *ctx, int M, int N, int K, int tri, int ktri, i
 /* on != 0: every later ovp_msckf_update of this context builds its point and plane systems with the one-block-per-feature kernel and
  * the dense stacked Gram matrix, also when all its tracks fit the warp-per-feature path (at most 32 measurements) */
 int ovp_debug_force_dense_features(ovp_ctx *ctx, int on);
+/* on != 0: every later compressed update of this context forms M = P[:, cols] L and S = L^T M[cols, :] + I with two GEMM launches after
+ * the factorisation of its Gram matrix, instead of inside that factorisation launch */
+int ovp_debug_unfused_update_products(ovp_ctx *ctx, int on);
+/* one factorisation of the lower triangle of G ((nc + 1) x (nc + 1), column-major) over its leading npiv columns with pivot tolerance
+ * tol, forming the update products in the same launch: with L = rows [0, nc) of the factor, M = P[:, cols] L (N x npiv) and the lower
+ * tiles of S = L^T M[cols, :] + I (npiv x npiv; the 64 x 64 tiles on and below the diagonal are written, S_out's other entries are kept).  P is N x N, cols holds nc indices into it.
+ * L_out receives the factor's (nc + 1) x npiv columns. */
+int ovp_debug_chol_products(ovp_ctx *ctx, const double *G, int nc, int npiv, double tol, const double *P, int N, const int *cols,
+                            double *L_out, double *M_out, double *S_out);
 
 #ifdef __cplusplus
 }

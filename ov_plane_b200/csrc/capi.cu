@@ -344,10 +344,10 @@ int ovp_create(const ovp_state_options *opt, int device, int max_state, int max_
   OVP_CUDA(cudaMalloc(&c->cf_diag0, (size_t)c->cf_maxT * 64 * sizeof(double)));
   OVP_CUDA(cudaMemset(c->cf_diag0, 0, (size_t)c->cf_maxT * 64 * sizeof(double)));
   OVP_CUDA(cudaMalloc(&c->cf_flags, (size_t)(3 * c->cf_maxT + c->cf_maxT * c->cf_maxT) * sizeof(int)));
-  OVP_CUDA(cudaMalloc(&c->cf_ctrl, 4 * sizeof(int)));
+  OVP_CUDA(cudaMalloc(&c->cf_ctrl, (4 + c->cf_maxT) * sizeof(int))); // epoch, finished CTAs, product queue head, M done per column block
   OVP_CUDA(cudaMemset(c->cf_linv, 0, (size_t)c->cf_maxT * 4096 * sizeof(double)));
   OVP_CUDA(cudaMemset(c->cf_flags, 0, (size_t)(3 * c->cf_maxT + c->cf_maxT * c->cf_maxT) * sizeof(int)));
-  OVP_CUDA(cudaMemset(c->cf_ctrl, 0, 4 * sizeof(int)));
+  OVP_CUDA(cudaMemset(c->cf_ctrl, 0, (4 + c->cf_maxT) * sizeof(int)));
   OVP_CUDA(cudaMalloc(&c->dM, (size_t)c->Nmax * c->Rcap * sizeof(double)));
   OVP_CUDA(cudaMalloc(&c->dY, (size_t)c->Nmax * c->Rcap * sizeof(double)));
   OVP_CUDA(cudaMalloc(&c->dHT, (size_t)c->Rcap * c->Rcap * sizeof(double)));

@@ -844,10 +844,7 @@ int ovp_msckf_update_gathered(ovp_ctx *h, const double *d_blocks, int G, const i
   st = gram_of_stacked(c, rows, nc1, ld);
   if (st)
     return st;
-  st = chol_partial(c, c->wsG.S, c->wsG.cap, nc1, n, c->gram_tol);
-  if (st)
-    return st;
-  st = ekf_update_core(c, c->dcols, n, mv(c->wsG.S, c->wsG.cap), n, c->wsG.S + (nc1 - 1), nullptr, -1.0, nullptr, nullptr, true, c->wsG.cap, false, true);
+  st = gram_factor_update(c, c->dcols, n, n, c->gram_tol, -1.0, nullptr, nullptr, false);
   if (st)
     return st;
   return check_status_flags(c);

@@ -190,3 +190,56 @@ extern "C" int ovp_debug_force_dense_features(ovp_ctx *h, int on) {
   h->c.force_dense_features = on != 0;
   return OVP_OK;
 }
+
+// Test hook (tests/test_gpu_fused_products.py): on != 0 sends every later compressed update of this context through the factorisation
+// and two GEMM launches for M and S, instead of the factorisation that forms them; the plan signature includes the setting.  Not part of
+// the ABI in include/ovp.h.
+extern "C" int ovp_debug_unfused_update_products(ovp_ctx *h, int on) {
+  h->c.unfused_update_products = on != 0;
+  return OVP_OK;
+}
+
+// Test hook (tests/test_gpu_fused_products.py): one factorisation launch that also forms the update products.  G: (nc + 1) x (nc + 1)
+// lower triangle, column-major, factored over its leading npiv columns with pivot tolerance tol; P: N x N, column-major; cols: nc state
+// indices.  L_out: (nc + 1) x npiv, M_out: N x npiv, S_out: npiv x npiv (lower triangle written, the rest left as passed in).  Not part of
+// the ABI in include/ovp.h.
+extern "C" int ovp_debug_chol_products(ovp_ctx *h, const double *G, int nc, int npiv, double tol, const double *P, int N, const int *cols,
+                                       double *L_out, double *M_out, double *S_out) {
+  Ctx *c = ovp::enter(h);
+  const int n = nc + 1;
+  if (n > c->wsG.cap || npiv > c->wsS.cap || N > c->Nmax || npiv > nc || N < 1 || npiv < 1)
+    return fail(c, OVP_ERR_CAPACITY, "debug_chol_products: too large");
+  const int ldp = (N + 1) & ~1;
+  char *buf = nullptr;
+  OVP_CUDA(cudaMalloc(&buf, (size_t)ldp * N * sizeof(double) + (size_t)nc * sizeof(int)));
+  double *dP = (double *)buf;
+  int *dcols = (int *)(dP + (size_t)ldp * N);
+  int st = OVP_OK;
+  auto run = [&]() -> int {
+    const int ldg = c->wsG.cap, lds = c->wsS.cap;
+    OVP_CUDA(cudaMemsetAsync(c->wsG.S, 0, (size_t)ldg * ldg * sizeof(double), c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(c->wsG.S, (size_t)ldg * sizeof(double), G, (size_t)n * sizeof(double), (size_t)n * sizeof(double), n,
+                               cudaMemcpyHostToDevice, c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(dP, (size_t)ldp * sizeof(double), P, (size_t)N * sizeof(double), (size_t)N * sizeof(double), N,
+                               cudaMemcpyHostToDevice, c->stream));
+    OVP_CUDA(cudaMemcpyAsync(dcols, cols, (size_t)nc * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(c->wsS.S, (size_t)lds * sizeof(double), S_out, (size_t)npiv * sizeof(double), (size_t)npiv * sizeof(double),
+                               npiv, cudaMemcpyHostToDevice, c->stream));
+    const CholProducts pr{dP, dcols, c->dM, c->wsS.S, ldp, N, nc, c->Nmax, lds};
+    int s = chol_fused(c, c->wsG.S, ldg, n, npiv, tol, nullptr, 0, 0, nullptr, 1, nullptr, 0, nullptr, -1.0, nullptr, nullptr, nullptr, &pr);
+    if (s)
+      return s;
+    OVP_CUDA(cudaGetLastError());
+    OVP_CUDA(cudaMemcpy2DAsync(L_out, (size_t)n * sizeof(double), c->wsG.S, (size_t)ldg * sizeof(double), (size_t)n * sizeof(double), npiv,
+                               cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(M_out, (size_t)N * sizeof(double), c->dM, (size_t)c->Nmax * sizeof(double), (size_t)N * sizeof(double), npiv,
+                               cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(S_out, (size_t)npiv * sizeof(double), c->wsS.S, (size_t)lds * sizeof(double), (size_t)npiv * sizeof(double),
+                               npiv, cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaStreamSynchronize(c->stream));
+    return OVP_OK;
+  };
+  st = run();
+  cudaFree(buf);
+  return st;
+}

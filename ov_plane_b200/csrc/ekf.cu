@@ -255,7 +255,7 @@ int join_side_stream(Ctx *c) {
 }
 
 int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const double *d_z, const double *d_Rdiag, double gate_thresh,
-                    int *d_gate_flag, double *d_chi2, bool apply, int zstride, bool defer_join, bool ht_lower) {
+                    int *d_gate_flag, double *d_chi2, bool apply, int zstride, bool defer_join, bool ht_lower, bool products_done) {
   if (rr <= 0 || nc <= 0)
     return OVP_OK;
   {
@@ -272,13 +272,13 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
   }
   const int N = c->N;
   // 1. M = P[:, cols] * HT        (N x rr)
-  {
+  if (!products_done) {
     GemmProblem p = make_problem(N, rr, nc, mv(c->dP, c->ldP, 0, nullptr, d_cols), HT, c->dM, c->Nmax);
     p.ktri = ht_lower ? 1 : 0; // H^T = L (the compression's Cholesky factor): column j is zero above row j
     launch_gemm1(c, p);
   }
   // 2. S = HT^T * M[cols, :] + R  (lower part)
-  {
+  if (!products_done) {
     MatView HTt = HT;
     HTt.trans ^= 1;
     GemmProblem p = make_problem(rr, rr, nc, HTt, mv(c->dM, c->Nmax, 0, d_cols, nullptr), c->wsS.S, c->wsS.cap);
@@ -333,6 +333,30 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
   if (!defer_join)
     return join_side_stream(c);
   return OVP_OK;
+}
+
+int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, double gate_thresh, int *d_gate_flag, double *d_chi2,
+                       bool defer_join) {
+  const int nc1 = nc + 1;
+  const MatView L = mv(c->wsG.S, c->wsG.cap);
+  const double *z = c->wsG.S + nc; // row nc of the factor, read in place (stride wsG.cap)
+  bool fused = !c->unfused_update_products && c->N > 0;
+  if (fused) {
+    if (npiv > c->wsS.cap || nc > c->Rcap)
+      return fail(c, OVP_ERR_CAPACITY, "ekf_update: system %d x %d exceeds capacity %d", npiv, nc, c->Rcap);
+    int st = join_side_stream(c); // the factorisation launch reads P for M = P[:, cols] L
+    if (st)
+      return st;
+    const CholProducts pr{c->dP, d_cols, c->dM, c->wsS.S, c->ldP, c->N, nc, c->Nmax, c->wsS.cap};
+    st = chol_fused(c, c->wsG.S, c->wsG.cap, nc1, npiv, tol, nullptr, 0, 0, nullptr, 1, nullptr, 0, nullptr, -1.0, nullptr, nullptr, nullptr, &pr);
+    if (st)
+      return st;
+  } else {
+    int st = chol_partial(c, c->wsG.S, c->wsG.cap, nc1, npiv, tol);
+    if (st)
+      return st;
+  }
+  return ekf_update_core(c, d_cols, nc, L, npiv, z, nullptr, gate_thresh, d_gate_flag, d_chi2, true, c->wsG.cap, defer_join, true, fused);
 }
 
 } // namespace ovp

@@ -51,6 +51,7 @@ struct Ctx {
   bool use_graphs = true;    // replay the static launch sequence of a prepared batch as a CUDA graph
   double gram_tol = 1e-11;   // zero-pivot rule of the Gram Cholesky, relative to the column's original diagonal (ovp_set_rank_tolerance)
   bool force_dense_features = false; // MSCKF batches take the one-block-per-feature kernel and the dense stack (ovp_debug_force_dense_features)
+  bool unfused_update_products = false; // compressed updates form M and S with two GEMM launches (ovp_debug_unfused_update_products)
 
   // --- State mirror -------------------------------------------------------------------------------------------
   int Nmax = 0, ldP = 0, N = 0;
@@ -163,8 +164,17 @@ int fail(Ctx *c, int status, const char *fmt, ...);
   } while (0)
 
 // ---- linalg.cu ---------------------------------------------------------------------------------------------------
+// The two products of a compressed update, formed inside the factorisation of its Gram matrix (cholfused.cu): with L = rows [0, nc) of
+// the factor, M = P[:, cols] L (N x npiv, ld ldm) and the lower tiles of S = L^T M[cols, :] + I (npiv x npiv, ld lds).  ldp is even.
+struct CholProducts {
+  const double *P;
+  const int *cols;
+  double *M, *S;
+  int ldp, N, nc, ldm, lds;
+};
 int chol_fused(Ctx *c, double *A, int ld, int n, int npiv, double tol, const double *M, int ldm, int mrows, const double *z, int zstride,
-               double *Y, int ldy, double *w, double gate_thresh, double *chi2, int *gate_flag, long long *dbg = nullptr);
+               double *Y, int ldy, double *w, double gate_thresh, double *chi2, int *gate_flag, long long *dbg = nullptr,
+               const CholProducts *prod = nullptr);
 // every tile CTA of one chol_fused launch must be co-resident: the tile CTAs a factorisation of the leading npiv columns of an n x n
 // system needs, how many the device holds, and the widest full factorisation (a multiple of 64) that fits
 int chol_fused_tiles(int n, int npiv);
@@ -189,8 +199,14 @@ void launch_fill(Ctx *c, double *p, size_t n, double v);
 // nc state indices).  z: rr.  Rdiag: rr or nullptr (identity).  If gate_thresh >= 0, chi2 = z^T S^-1 z is compared with
 // it on the device and the update is skipped when larger (flag written to d_gate_flag, chi2 to d_chi2).  ht_lower: HT(k, j) == 0 for k < j
 // (HT is the lower Cholesky factor of the compression) - the two products skip the structural zeros.
+// products_done: M = P[:, cols] HT (in dM) and S = HT^T M[cols, :] + R (in wsS) are already formed; steps 1-2 are skipped.
 int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const double *d_z, const double *d_Rdiag, double gate_thresh,
-                    int *d_gate_flag, double *d_chi2, bool apply = true, int zstride = 1, bool defer_join = false, bool ht_lower = false);
+                    int *d_gate_flag, double *d_chi2, bool apply = true, int zstride = 1, bool defer_join = false, bool ht_lower = false,
+                    bool products_done = false);
+// The compressed update: factor the Gram matrix in wsG (nc + 1 columns, z last; pivots on the leading npiv) and update with H^T = L
+// (rows [0, nc)), z = row nc of the factor, R = I.  The factorisation launch also forms M and S.
+int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, double gate_thresh, int *d_gate_flag, double *d_chi2,
+                       bool defer_join);
 int join_side_stream(Ctx *c); // make the main stream wait for the side stream's covariance downdate (no-op when nothing is pending)
 int upload_var_table(Ctx *c);
 int sync_host_values(Ctx *c);
