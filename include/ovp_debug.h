@@ -3,8 +3,9 @@
  * These entry points exist only in ov_plane_b200/lib/libovp_debug.so (the product sources compiled with -DOVP_DEBUG); the
  * product library libovp.so does not export them.  They let tools/microbench_chol.py time the fused Cholesky, let
  * tests/test_gpu_cholfused.py / tests/test_gpu_gemm.py / tests/test_gpu_gemm_split.py unit-test chol_fused_kernel and the DMMA GEMM against NumPy on arbitrary
- * matrices, let tests/test_gpu_numerics.py run one batch through both MSCKF feature paths, and let tests/test_gpu_fused_products.py check the
- * update products formed inside the Gram factorisation and run the update both with and without them. */
+ * matrices, let tests/test_gpu_numerics.py run one batch through both MSCKF feature paths, let tests/test_gpu_fused_products.py check the
+ * update products formed inside the Gram factorisation and run the update both with and without them, and let
+ * tests/test_gpu_compression.py check the compressed update's Gram matrix, zero-pivot rule and innovation gate element by element. */
 #ifndef OVP_DEBUG_H
 #define OVP_DEBUG_H
 #include "ovp.h"
@@ -19,6 +20,12 @@ int ovp_debug_chol_fused(ovp_ctx *ctx, int n, int mrows, int iters, double *out,
  * when M is given, solve Y = M L^-T (mrows x npiv) and w = L^-1 z */
 int ovp_debug_chol_solve(ovp_ctx *ctx, const double *A, int n, int npiv, double tol, const double *M, int mrows, const double *z,
                          double *L_out, double *Y_out, double *w_out);
+/* ovp_debug_chol_solve with the innovation launch's gate (tests/test_gpu_compression.py): the same launch also forms chi2 = |w|^2
+ * (chi2_out) and the gate flag (gate_out: 1 when gate_thresh < 0 or chi2 <= gate_thresh, else 0).  z holds npiv values; the launch
+ * reads them with stride 1 (zstride = 1) or in place as a row of a column-major workspace, with the stride of the compressed update
+ * (zstride = 0).  chi2_out and gate_out may be NULL. */
+int ovp_debug_chol_solve_gated(ovp_ctx *ctx, const double *A, int n, int npiv, double tol, const double *M, int mrows, const double *z,
+                               int zstride, double gate_thresh, double *L_out, double *Y_out, double *w_out, double *chi2_out, int *gate_out);
 /* one product C = alpha * A B + beta * C (+ diagonal) through the DMMA GEMM (tests/test_gpu_gemm.py).  Host matrices are column-major:
  * A is a_rows x a_cols, logical A (M x K) = A, or A^T when a_trans; B is b_rows x b_cols, logical B (K x N) = B, or B^T when b_trans.
  * akidx / bkidx (length K, or NULL) gather the contraction index of A / B.  C is ldc x N, updated in place.  diag_add (length
@@ -44,6 +51,17 @@ int ovp_debug_unfused_update_products(ovp_ctx *ctx, int on);
  * L_out receives the factor's (nc + 1) x npiv columns. */
 int ovp_debug_chol_products(ovp_ctx *ctx, const double *G, int nc, int npiv, double tol, const double *P, int N, const int *cols,
                             double *L_out, double *M_out, double *S_out);
+/* prepare a feature batch as ovp_msckf_update does and run the first non-empty plan of its launch order (planes in ascending id, then the
+ * point update) up to its Gram matrix G = [H_o r_o]^T [H_o r_o] of the nullspace-projected system; the state is left as it was.  G_out
+ * (gcap * gcap doubles) receives all of G, nc1 x nc1 column-major: the ncx x columns (calibration, then 6 per clone), for a plane its
+ * 3 H_cp columns, the residual last.  info[8] = {nc1, ncal, ncx, point plan, nsel, warp-per-feature path, plane slot, plane in the
+ * state}.  cols_out (gcap): state index of every x column; sel_out (F): the nsel features of the plan; feat_status / feat_chi2 (F): the
+ * per-feature status words after the plan's feature kernel (point plan: 1 accepted, 0 rejected by the gate).  raw_out (NULL, or 72
+ * doubles per measurement of the batch): the raw whitened rows the feature kernel built, per measurement 3 rows of 24 doubles: the two
+ * bearing rows [0,3) H_f, [3,9) H_clone, [9, 9 + ncal) calibration, [23] r, then (plane plans) the point-on-plane row [0,3) H_f,
+ * [9,12) H_cp, [23] r.  A plan that updates without compression has no Gram matrix: OVP_ERR_BAD_ARGS. */
+int ovp_debug_msckf_gram(ovp_ctx *ctx, const ovp_feature_batch *b, const ovp_updater_options *opt, int gcap, double *G_out, int *info,
+                         int *cols_out, int *sel_out, int *feat_status, double *feat_chi2, double *raw_out);
 
 #ifdef __cplusplus
 }

@@ -1,7 +1,8 @@
 // TEST / TUNING HOOKS — compiled only into libovp_debug.so (-DOVP_DEBUG), never into the product library libovp.so.
 // Declared in include/ovp_debug.h.  Used by tools/microbench_chol.py (phase timeline of the fused Cholesky), by
-// tests/test_gpu_cholfused.py and tests/test_gpu_gemm.py (unit tests of chol_fused_kernel and the DMMA GEMM against NumPy) and by
-// tests/test_gpu_numerics.py (the block-sparse feature path against the dense stack on the same batch).
+// tests/test_gpu_cholfused.py and tests/test_gpu_gemm.py (unit tests of chol_fused_kernel and the DMMA GEMM against NumPy), by
+// tests/test_gpu_numerics.py (the block-sparse feature path against the dense stack on the same batch) and by tests/test_gpu_compression.py
+// (the compressed update's Gram matrix, zero-pivot rule and innovation gate against long-double references).
 #include "ovp_internal.h"
 using namespace ovp;
 
@@ -146,25 +147,41 @@ extern "C" int ovp_debug_gemm_split(ovp_ctx *h, int M, int N, int K, int tri, in
   return OVP_OK;
 }
 
-// Test hook for the fused Cholesky (tests/test_gpu_cholfused.py): factor a host matrix (lower triangle of A, n x n, column-major)
-// over its leading npiv columns with pivot tolerance tol and, when M is given, solve Y = M L^-T (mrows x npiv) and w = L^-1 z.
-// Not part of the ABI in include/ovp.h.
-extern "C" int ovp_debug_chol_solve(ovp_ctx *h, const double *A, int n, int npiv, double tol, const double *M, int mrows, const double *z,
-                                    double *L_out, double *Y_out, double *w_out) {
+// Test hook for the innovation launch of the fused Cholesky (tests/test_gpu_compression.py): factor a host matrix (lower triangle of A,
+// n x n, column-major) over its leading npiv columns with pivot tolerance tol and, when M is given, solve Y = M L^-T (mrows x npiv) and
+// w = L^-1 z, and form chi2 = |w|^2 and the gate flag of gate_thresh in the same launch.  z (npiv values) is read on the device with
+// stride zstride: 1 from a vector of its own, 0 in place in a column-major workspace of leading dimension wsG.cap, the layout of the
+// compressed update (gram_factor_update reads z as the last row of the Gram factor); the rest of that workspace holds NaNs.  Not part of
+// the ABI in include/ovp.h.
+extern "C" int ovp_debug_chol_solve_gated(ovp_ctx *h, const double *A, int n, int npiv, double tol, const double *M, int mrows,
+                                          const double *z, int zstride, double gate_thresh, double *L_out, double *Y_out, double *w_out,
+                                          double *chi2_out, int *gate_out) {
   Ctx *c = ovp::enter(h);
-  if (n > c->wsS.cap || mrows > c->Nmax || npiv > n)
+  if (n > c->wsS.cap || mrows > c->Nmax || npiv > n || npiv > c->wsG.cap)
     return fail(c, OVP_ERR_CAPACITY, "debug_chol_solve: too large");
+  if (zstride != 0 && zstride != 1)
+    return fail(c, OVP_ERR_BAD_ARGS, "debug_chol_solve: zstride must be 0 or 1");
   const int ld = c->wsS.cap;
   OVP_CUDA(cudaMemsetAsync(c->wsS.S, 0, (size_t)ld * ld * sizeof(double), c->stream));
   OVP_CUDA(cudaMemcpy2DAsync(c->wsS.S, (size_t)ld * sizeof(double), A, (size_t)n * sizeof(double), (size_t)n * sizeof(double), n,
                              cudaMemcpyHostToDevice, c->stream));
+  double *dz = nullptr;
+  int zs = 1;
   if (M) {
     OVP_CUDA(cudaMemcpy2DAsync(c->dM, (size_t)c->Nmax * sizeof(double), M, (size_t)mrows * sizeof(double), (size_t)mrows * sizeof(double),
                                npiv, cudaMemcpyHostToDevice, c->stream));
-    OVP_CUDA(cudaMemcpyAsync(c->dvec + c->Rcap, z, (size_t)npiv * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    if (zstride == 1) {
+      dz = c->dvec + c->Rcap;
+      OVP_CUDA(cudaMemcpyAsync(dz, z, (size_t)npiv * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    } else { // row npiv - 1 of the Gram workspace, as row nc of the compressed update's factor (all-ones bytes: NaN everywhere else)
+      zs = c->wsG.cap;
+      dz = c->wsG.S + (npiv - 1);
+      OVP_CUDA(cudaMemsetAsync(c->wsG.S, 0xff, (size_t)zs * zs * sizeof(double), c->stream));
+      OVP_CUDA(cudaMemcpy2DAsync(dz, (size_t)zs * sizeof(double), z, sizeof(double), sizeof(double), npiv, cudaMemcpyHostToDevice, c->stream));
+    }
   }
-  int st = chol_fused(c, c->wsS.S, ld, n, npiv, tol, M ? c->dM : nullptr, c->Nmax, mrows, M ? c->dvec + c->Rcap : nullptr, 1, c->dY, c->Nmax, c->dvec, -1.0,
-                      c->dscal + 8, nullptr);
+  int st = chol_fused(c, c->wsS.S, ld, n, npiv, tol, M ? c->dM : nullptr, c->Nmax, mrows, dz, zs, c->dY, c->Nmax, c->dvec, gate_thresh,
+                      c->dscal + 8, c->dflags + 3);
   if (st)
     return st;
   OVP_CUDA(cudaMemcpy2DAsync(L_out, (size_t)n * sizeof(double), c->wsS.S, (size_t)ld * sizeof(double), (size_t)n * sizeof(double), n,
@@ -173,6 +190,10 @@ extern "C" int ovp_debug_chol_solve(ovp_ctx *h, const double *A, int n, int npiv
     OVP_CUDA(cudaMemcpy2DAsync(Y_out, (size_t)mrows * sizeof(double), c->dY, (size_t)c->Nmax * sizeof(double), (size_t)mrows * sizeof(double),
                                npiv, cudaMemcpyDeviceToHost, c->stream));
     OVP_CUDA(cudaMemcpyAsync(w_out, c->dvec, (size_t)npiv * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    if (chi2_out)
+      OVP_CUDA(cudaMemcpyAsync(chi2_out, c->dscal + 8, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    if (gate_out)
+      OVP_CUDA(cudaMemcpyAsync(gate_out, c->dflags + 3, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   }
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   int info = 0;
@@ -182,6 +203,13 @@ extern "C" int ovp_debug_chol_solve(ovp_ctx *h, const double *A, int n, int npiv
     return fail(c, OVP_ERR_NOT_POSITIVE_DEFINITE, "debug_chol_solve: matrix not positive definite (strict mode)");
   }
   return OVP_OK;
+}
+
+// Test hook for the fused Cholesky (tests/test_gpu_cholfused.py, tests/test_gpu_fused_products.py): ovp_debug_chol_solve_gated with z
+// read from a vector of its own and no gate.  Not part of the ABI in include/ovp.h.
+extern "C" int ovp_debug_chol_solve(ovp_ctx *h, const double *A, int n, int npiv, double tol, const double *M, int mrows, const double *z,
+                                    double *L_out, double *Y_out, double *w_out) {
+  return ovp_debug_chol_solve_gated(h, A, n, npiv, tol, M, mrows, z, 1, -1.0, L_out, Y_out, w_out, nullptr, nullptr);
 }
 
 // Test hook (tests/test_gpu_numerics.py): on != 0 sends every later MSCKF batch of this context through the one-block-per-feature kernel
@@ -241,5 +269,70 @@ extern "C" int ovp_debug_chol_products(ovp_ctx *h, const double *G, int nc, int 
   };
   st = run();
   cudaFree(buf);
+  return st;
+}
+
+// Test hook (tests/test_gpu_compression.py): prepare a feature batch as ovp_msckf_update does and run the first non-empty plan of its
+// launch order (a plane plan first if the batch has planes, otherwise the point plan) up to its Gram matrix G = D - Y^T Y; nothing after
+// it runs, so the state is left as it was.  Eager launches.  G_out (gcap x gcap, column-major, leading dimension nc1) receives all of G.
+// info: [0] nc1, [1] ncal, [2] ncx (x columns; H_cp, when present, sits at ncx .. ncx + 2 and the residual at nc1 - 1), [3] point plan,
+// [4] selected features nsel, [5] warp-per-feature path, [6] plane slot, [7] plane in the state.  cols_out (gcap): compact column -> state
+// index of the x columns; sel_out (F): the plan's features; feat_status / feat_chi2 (F): the per-feature status words after the plan's
+// feature kernel.  raw_out (optional, 3 * OVP_RAW_ROW doubles per measurement, OVP_RAW_ROW in features.cu): the raw whitened rows the
+// feature kernel built.  A plan that goes straight into the update (no compression) has no Gram matrix: OVP_ERR_BAD_ARGS.  Not part of
+// the ABI in include/ovp.h.
+extern "C" int ovp_debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, const ovp_updater_options *opt, int gcap, double *G_out,
+                                    int *info, int *cols_out, int *sel_out, int *feat_status, double *feat_chi2, double *raw_out) {
+  Ctx *c = ovp::enter(h);
+  if (!b || !opt || b->F <= 0)
+    return fail(c, OVP_ERR_BAD_ARGS, "debug_msckf_gram: empty batch");
+  int st = msckf_prepare(c, b, opt, nullptr);
+  if (st)
+    return st;
+  Prepared &P = *(Prepared *)c->prep;
+  const size_t nraw = (size_t)3 * OVP_RAW_ROW * std::max(P.M, 1);
+  double *draw = nullptr;
+  if (raw_out) {
+    OVP_CUDA(cudaMalloc(&draw, nraw * sizeof(double)));
+    OVP_CUDA(cudaMemsetAsync(draw, 0, nraw * sizeof(double), c->stream));
+  }
+  c->dbg_raw = draw;
+  c->dbg_gram_stop = true;
+  c->dbg_gram_plan = -1;
+  st = msckf_launch_body(c, true);
+  c->dbg_raw = nullptr;
+  c->dbg_gram_stop = false;
+  P.valid = false; // the next update prepares its batch again (this one stopped half way)
+  auto run = [&]() -> int {
+    if (st)
+      return st;
+    OVP_CUDA(cudaStreamSynchronize(c->stream));
+    if (c->dbg_gram_plan < 0)
+      return fail(c, OVP_ERR_BAD_ARGS, "debug_msckf_gram: the first plan goes straight into the update, without a Gram matrix");
+    const UpdatePlan &pl = P.plans[c->dbg_gram_plan];
+    const int ncx = (int)pl.cols.size(), nc1 = pl.is_point ? ncx + 1 : ncx + 4;
+    if (nc1 > gcap)
+      return fail(c, OVP_ERR_CAPACITY, "debug_msckf_gram: %d columns, room for %d", nc1, gcap);
+    const int ncal = (c->opt.do_calib_camera_pose ? 6 : 0) + (c->opt.do_calib_camera_intrinsics ? 8 : 0);
+    const int v[8] = {nc1, ncal, ncx, pl.is_point ? 1 : 0, (int)pl.feats.size(), P.fast ? 1 : 0, pl.plane_slot, pl.in_state ? 1 : 0};
+    std::memcpy(info, v, sizeof(v));
+    std::memcpy(cols_out, pl.cols.data(), ncx * sizeof(int));
+    std::memcpy(sel_out, pl.feats.data(), pl.feats.size() * sizeof(int));
+    OVP_CUDA(cudaMemcpy2DAsync(G_out, (size_t)nc1 * sizeof(double), c->wsG.S, (size_t)c->wsG.cap * sizeof(double), (size_t)nc1 * sizeof(double),
+                               nc1, cudaMemcpyDeviceToHost, c->stream));
+    if (raw_out)
+      OVP_CUDA(cudaMemcpyAsync(raw_out, draw, nraw * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    std::vector<int> flag;
+    std::vector<double> chi2;
+    int s = read_feature_status(c, P.F, (const char *)c->d_batch, P.o_flag, P.o_chi, flag, chi2); // synchronises
+    if (s)
+      return s;
+    std::memcpy(feat_status, flag.data(), P.F * sizeof(int));
+    std::memcpy(feat_chi2, chi2.data(), P.F * sizeof(double));
+    return OVP_OK;
+  };
+  st = run();
+  if (draw)
+    cudaFree(draw);
   return st;
 }

@@ -17,6 +17,12 @@
 
 namespace ovp {
 
+#ifdef OVP_DEBUG
+// Raw whitened blocks of the MSCKF feature kernels as they hold them (ovp_debug_msckf_gram, libovp_debug.so only).  Measurement g of the
+// batch owns 3 rows of OVP_RAW_ROW doubles from raw[g * 3 * OVP_RAW_ROW]: its two bearing rows, [0,3) H_f, [3,9) H_clone,
+// [9, 9 + ncal) calibration, [23] r; in plane mode its point-on-plane row, [0,3) H_f, [9,12) H_cp, [23] r.  Entries not named are left.
+#define OVP_RAW_ROW 24
+#endif
 struct FeatArgs {
   const int *meas_offset;
   const int *meas_clone;
@@ -45,6 +51,9 @@ struct FeatArgs {
   int col_cp, col_res;    // stacked-system columns of H_cp (3, mode 1) and of the residual
   double *Hs;
   int ldHs;
+#ifdef OVP_DEBUG
+  double *raw; // ovp_debug_msckf_gram: the raw whitened blocks of every feature (layout OVP_RAW_* above), nullptr: none
+#endif
   const double *chi2_table;
   int chi2_n;
   double chi2_mult;
@@ -228,6 +237,16 @@ __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
         A[(size_t)(cb + 6 * k + j) * lda + r] = Hcl[6 * i + j];
       A[(size_t)c_res * lda + r] = res[i];
     }
+#ifdef OVP_DEBUG
+    if (a.raw && a.mode != 2) // the rows just written to A, in the layout of OVP_RAW_ROW
+      for (int i = 0; i < 2; i++) {
+        double *rw = a.raw + ((size_t)(m0 + k) * 3 + i) * OVP_RAW_ROW;
+        for (int j = 0; j < 3 + cf; j++)
+          if (j < 3 + ncal || (j >= 3 + ncal + 6 * k && j < 3 + ncal + 6 * k + 6))
+            rw[j < 3 ? j : (j < 3 + ncal ? j + 6 : j - ncal - 6 * k)] = A[(size_t)j * lda + 2 * k + i];
+        rw[OVP_RAW_ROW - 1] = A[(size_t)c_res * lda + 2 * k + i];
+      }
+#endif
     const int idc = a.var_id[hcl];
     for (int j = 0; j < 6; j++)
       gid[3 + ncal + 6 * k + j] = idc + j;
@@ -248,6 +267,16 @@ __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
         A[(size_t)(c_cp + j) * lda + r] = pHcp[j];
       }
       A[(size_t)c_res * lda + r] = pr;
+#ifdef OVP_DEBUG
+      if (a.raw && a.mode == 1) {
+        double *rw = a.raw + ((size_t)(m0 + k) * 3 + 2) * OVP_RAW_ROW;
+        for (int j = 0; j < 3; j++) {
+          rw[j] = A[(size_t)j * lda + r];
+          rw[9 + j] = A[(size_t)(c_cp + j) * lda + r];
+        }
+        rw[OVP_RAW_ROW - 1] = A[(size_t)c_res * lda + r];
+      }
+#endif
     }
   }
   if (tid == 0) {

@@ -52,6 +52,13 @@ struct Ctx {
   double gram_tol = 1e-11;   // zero-pivot rule of the Gram Cholesky, relative to the column's original diagonal (ovp_set_rank_tolerance)
   bool force_dense_features = false; // MSCKF batches take the one-block-per-feature kernel and the dense stack (ovp_debug_force_dense_features)
   bool unfused_update_products = false; // compressed updates form M and S with two GEMM launches (ovp_debug_unfused_update_products)
+#ifdef OVP_DEBUG
+  // ovp_debug_msckf_gram: the feature kernels write their raw blocks to dbg_raw (when set), and with dbg_gram_stop the MSCKF launch
+  // returns right after the first Gram matrix it forms, recording that plan's index in dbg_gram_plan
+  double *dbg_raw = nullptr;
+  bool dbg_gram_stop = false;
+  int dbg_gram_plan = -1;
+#endif
 
   // --- State mirror -------------------------------------------------------------------------------------------
   int Nmax = 0, ldP = 0, N = 0;
