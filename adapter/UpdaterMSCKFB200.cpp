@@ -3,13 +3,15 @@
 // (cleaning the tracks, grouping the features by plane, flagging what was consumed); every numerical stage is one call into the C ABI:
 //   UpdaterMSCKF.cpp:142-194  triangulation                      -> ovp_triangulate_features
 //   :262-360                  plane hypotheses + refinement       -> ovp_plane_fitting, ovp_optimize_plane (all planes of the frame in one batch)
-//   :407-828                  plane updates, gates, compression,  -> ovp_msckf_update (one call; the chain of dependent updates stays on the device)
-//                             StateHelper::EKFUpdate
+//   :407-828                  plane updates, gates, compression,  -> ovp_msckf_update_landmarks (one call; the chain of dependent updates stays
+//                             StateHelper::EKFUpdate, with the        on the device; the library keeps _features_SLAM_to_PLANE of the members)
+//                             SLAM landmarks of out-of-state planes (:231-254)
 // The chi2 table (:57-62) is handed to the library once (ovp_set_chi2_table) by the code that creates the context.
 #include "update/UpdaterMSCKF.h"
 
 #include <cstdio>
 #include <cstdlib>
+#include <memory>
 #include <set>
 
 #include "feat/Feature.h"
@@ -110,11 +112,31 @@ void UpdaterMSCKF::update(std::shared_ptr<State> state, std::vector<std::shared_
   // 4. planes of this frame (:198-404): features grouped by plane id, in-state planes refine their features against the state's estimate,
   //    new planes get a RANSAC hypothesis and a joint refinement - all candidates of the frame in ONE batch per stage
   std::map<size_t, std::vector<std::shared_ptr<ov_core::Feature>>> plane_feats;
-  if (state->_options.use_plane_constraint && state->_options.use_plane_constraint_msckf) {
-    for (auto *vec : {&feature_vec, &feature_vec_extra})
-      for (auto &feat : *vec)
-        if (feat2plane.find(feat->featid) != feat2plane.end())
-          plane_feats[feat2plane.at(feat->featid)].push_back(feat);
+  std::set<ov_core::Feature *> slam_members; // SLAM landmarks as measurement-free features of their plane (:231-254)
+  if (state->_options.use_plane_constraint && (state->_options.use_plane_constraint_msckf || state->_options.use_plane_constraint_slamu)) {
+    if (state->_options.use_plane_constraint_msckf)
+      for (auto *vec : {&feature_vec, &feature_vec_extra})
+        for (auto &feat : *vec)
+          if (feat2plane.find(feat->featid) != feat2plane.end())
+            plane_feats[feat2plane.at(feat->featid)].push_back(feat);
+    if (state->_options.use_plane_constraint_slamu) {
+      std::set<size_t> slam_ids; // ascending featid, the std::map order of the reference's _features_SLAM
+      for (auto &kv : state->_features_SLAM)
+        slam_ids.insert(kv.first);
+      for (size_t featid : slam_ids) {
+        auto it = feat2plane.find(featid);
+        if (it == feat2plane.end() || state->_features_PLANE.count(it->second) || ovp_slam_plane_of(state->ctx, (int64_t)featid) == 0)
+          continue;
+        double value[16], fej[16]; // the device holds the current estimate
+        ck(state, ovp_var_get(state->ctx, ovp_slam_handle(state->ctx, (int64_t)featid), value, fej));
+        auto lm = std::make_shared<ov_core::Feature>();
+        lm->featid = featid;
+        for (int k = 0; k < 3; k++)
+          lm->p_FinG(k) = value[k];
+        slam_members.insert(lm.get());
+        plane_feats[it->second].push_back(lm);
+      }
+    }
   }
   std::map<size_t, Eigen::Vector3d> plane_estimates_cp_inG;
   std::vector<size_t> cand; // plane ids that go through the refinement, in std::map order
@@ -217,14 +239,23 @@ void UpdaterMSCKF::update(std::shared_ptr<State> state, std::vector<std::shared_
   std::set<ov_core::Feature *> in_main;
   for (auto &f : feature_vec)
     in_main.insert(f.get());
-  for (auto &kv : plane_feats) // features of feature_vec_extra that lie on a plane with an estimate take part in its update only
-    if (plane_estimates_cp_inG.count(kv.first))
-      for (auto &f : kv.second)
-        if (!in_main.count(f.get())) {
-          all.push_back(f);
-          for (int k = 0; k < 3; k++)
-            p_original.push_back(f->p_FinG(k));
-        }
+  // features of feature_vec_extra that lie on a plane with an estimate take part in its update only; landmarks that stayed on such a
+  // plane are members of its update
+  std::vector<int64_t> lm_featid, lm_planeid;
+  for (auto &kv : plane_feats) {
+    if (!plane_estimates_cp_inG.count(kv.first))
+      continue;
+    for (auto &f : kv.second) {
+      if (slam_members.count(f.get())) {
+        lm_featid.push_back((int64_t)f->featid);
+        lm_planeid.push_back((int64_t)kv.first);
+      } else if (!in_main.count(f.get())) {
+        all.push_back(f);
+        for (int k = 0; k < 3; k++)
+          p_original.push_back(f->p_FinG(k));
+      }
+    }
+  }
   Flat fl;
   std::vector<double> p;
   std::vector<int64_t> featid, planeid, plane_ids;
@@ -256,7 +287,8 @@ void UpdaterMSCKF::update(std::shared_ptr<State> state, std::vector<std::shared_
   b.plane_cp = plane_cp.data();
   ovp_updater_options uo = {_options.sigma_pix, _options.chi2_multipler};
   std::vector<int> feat_status(all.size()), plane_status(plane_ids.size() + 1);
-  ck(state, ovp_msckf_update(state->ctx, &b, &uo, feat_status.data(), nullptr, plane_status.data(), nullptr, nullptr, nullptr));
+  const ovp_plane_landmarks lm = {(int)lm_featid.size(), lm_featid.data(), lm_planeid.data()};
+  ck(state, ovp_msckf_update_landmarks(state->ctx, &b, &lm, &uo, feat_status.data(), nullptr, plane_status.data(), nullptr, nullptr, nullptr));
   // bookkeeping of the outcome: rejected features are deleted, features consumed by a passed plane update are reported as used (:640-659, :745-764)
   for (size_t i = 0; i < all.size(); i++) {
     if (feat_status[i] == 0)

@@ -186,6 +186,23 @@ typedef struct ovp_updater_options { /* UpdaterOptions.h:38-54 */
 int ovp_msckf_update(ovp_ctx *ctx, const ovp_feature_batch *batch, const ovp_updater_options *opt, int *feat_status,
                      double *feat_chi2, int *plane_status, double *plane_chi2, int *hx_order, int *hx_order_n);
 
+/* The same update with the in-state SLAM landmarks of use_plane_constraint_slamu (UpdaterMSCKF.cpp:231-254, 454-560, 626-639).
+ * The caller passes the feat2plane entries of its landmarks (n = 0: slamu off, the result is bit-identical to ovp_msckf_update);
+ * the library keeps the ones that join a plane: featid is in State::_features_SLAM, planeid names a plane of the batch that is NOT
+ * in the state, and _features_SLAM_to_PLANE[featid] is absent or non-zero.  Each member counts towards its plane's 4-feature
+ * rule (the plane still needs one batch feature) and adds one point-on-plane row with its 3 landmark columns as state columns
+ * (residual at the landmark's value, Jacobians at its first estimate when do_fej).  After the plane's gate the library sets
+ * _features_SLAM_to_PLANE[featid] to the plane id (pass) or 0 (fail).  Refused with OVP_ERR_BAD_ARGS before anything is
+ * launched: a member that is not GLOBAL_3D, a featid listed twice, a featid that is also a feature of the batch. */
+typedef struct ovp_plane_landmarks {
+  int n;
+  const int64_t *featid;  /* n */
+  const int64_t *planeid; /* n: feat2plane entry, 0 = not on a plane */
+} ovp_plane_landmarks;
+int ovp_msckf_update_landmarks(ovp_ctx *ctx, const ovp_feature_batch *batch, const ovp_plane_landmarks *landmarks,
+                               const ovp_updater_options *opt, int *feat_status, double *feat_chi2, int *plane_status,
+                               double *plane_chi2, int *hx_order, int *hx_order_n);
+
 /* UpdaterPlane::init_vio_plane from "plane linearisation points known" on (UpdaterPlane.cpp:297-481): every plane of the batch
  * that is NOT in the state (ascending id) and has >= 3 features is stacked (Jacobians with sigma_c * const_init_multi),
  * compressed and handed to StateHelper::initialize with const_init_chi2.  plane_status[i]: 1 initialised, 0 chi2-rejected,
@@ -339,6 +356,9 @@ int ovp_zupt_try_update(ovp_ctx *ctx, const ovp_zupt_options *opt, double timest
  * planning and the single host->device copy; launch = kernels only (asynchronous, repeatable: the state changes, the plan
  * does not); finish = device->host read of the gates and Hx_order.  ovp_msckf_update == prepare + launch + finish. */
 int ovp_msckf_prepare(ovp_ctx *ctx, const ovp_feature_batch *batch, const ovp_updater_options *opt);
+/* prepare of ovp_msckf_update_landmarks; the member list is part of the plan, and members' values are read on the device */
+int ovp_msckf_prepare_landmarks(ovp_ctx *ctx, const ovp_feature_batch *batch, const ovp_plane_landmarks *landmarks,
+                                const ovp_updater_options *opt);
 int ovp_msckf_launch(ovp_ctx *ctx);
 int ovp_msckf_finish(ovp_ctx *ctx, int *feat_status, double *feat_chi2, int *plane_status, double *plane_chi2, int *hx_order,
                      int *hx_order_n);

@@ -62,6 +62,11 @@ int ovp_debug_chol_products(ovp_ctx *ctx, const double *G, int nc, int npiv, dou
  * [9,12) H_cp, [23] r.  A plan that updates without compression has no Gram matrix: OVP_ERR_BAD_ARGS. */
 int ovp_debug_msckf_gram(ovp_ctx *ctx, const ovp_feature_batch *b, const ovp_updater_options *opt, int gcap, double *G_out, int *info,
                          int *cols_out, int *sel_out, int *feat_status, double *feat_chi2, double *raw_out);
+/* the same for ovp_msckf_update_landmarks: a plane plan's G also holds its landmark members' rows, their 3 columns each after the batch
+ * features' x columns (counted in ncx; cols_out gives their state indices) and before H_cp. */
+int ovp_debug_msckf_gram_landmarks(ovp_ctx *ctx, const ovp_feature_batch *b, const ovp_plane_landmarks *lm, const ovp_updater_options *opt,
+                                   int gcap, double *G_out, int *info, int *cols_out, int *sel_out, int *feat_status, double *feat_chi2,
+                                   double *raw_out);
 
 #ifdef __cplusplus
 }

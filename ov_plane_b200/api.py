@@ -34,6 +34,10 @@ class FeatureBatch(C.Structure):
                 ("plane_ids", C.c_void_p), ("plane_cp", C.c_void_p)]
 
 
+class PlaneLandmarks(C.Structure):
+    _fields_ = [("n", C.c_int), ("featid", C.c_void_p), ("planeid", C.c_void_p)]
+
+
 class UpdaterOptions(C.Structure):
     _fields_ = [("sigma_pix", C.c_double), ("chi2_multipler", C.c_double)]
 
@@ -371,6 +375,28 @@ class Context(object):
         self._ck(self.lib.ovp_msckf_update(self.h, C.byref(fb), C.byref(uo), _p(fs), _p(fc), _p(ps), _p(pc), _p(hx), C.byref(hxn)))
         return dict(feat_status=fs, feat_chi2=fc, plane_status=ps[:fb.nplanes], plane_chi2=pc[:fb.nplanes], hx_order=hx[:hxn.value].tolist())
 
+    @staticmethod
+    def _landmarks_struct(featid, planeid):
+        fid = np.ascontiguousarray(featid, dtype=np.int64).ravel()
+        pid = np.ascontiguousarray(planeid, dtype=np.int64).ravel()
+        if fid.shape != pid.shape:
+            raise ValueError("featid and planeid need one entry per landmark")
+        return PlaneLandmarks(len(fid), fid.ctypes.data, pid.ctypes.data), (fid, pid)
+
+    def msckf_update_landmarks(self, batch, lm_featid, lm_planeid, sigma_pix=1.0, chi2_mult=1.0):
+        """msckf_update with use_plane_constraint_slamu: (lm_featid[i], lm_planeid[i]) are the feat2plane entries of the caller's SLAM
+        landmarks; the ones on planes of the batch that are not in the state join those planes' updates."""
+        fb, keep = self._batch_struct(batch)
+        lm, keep_lm = self._landmarks_struct(lm_featid, lm_planeid)
+        uo = UpdaterOptions(sigma_pix, chi2_mult)
+        F, npl = fb.F, max(1, fb.nplanes)
+        fs, fc = np.zeros(F, dtype=np.int32), np.zeros(F)
+        ps, pc = np.zeros(npl, dtype=np.int32), np.zeros(npl)
+        hx, hxn = np.zeros(4096, dtype=np.int32), C.c_int(0)
+        self._ck(self.lib.ovp_msckf_update_landmarks(self.h, C.byref(fb), C.byref(lm), C.byref(uo), _p(fs), _p(fc), _p(ps), _p(pc), _p(hx),
+                                                     C.byref(hxn)))
+        return dict(feat_status=fs, feat_chi2=fc, plane_status=ps[:fb.nplanes], plane_chi2=pc[:fb.nplanes], hx_order=hx[:hxn.value].tolist())
+
     def plane_init(self, batch, sigma_pix=1.0, chi2_mult=1.0):
         fb, keep = self._batch_struct(batch)
         uo = UpdaterOptions(sigma_pix, chi2_mult)
@@ -541,6 +567,13 @@ class Context(object):
         self._prep_F, self._prep_np = fb.F, fb.nplanes
         uo = UpdaterOptions(sigma_pix, chi2_mult)
         self._ck(self.lib.ovp_msckf_prepare(self.h, C.byref(fb), C.byref(uo)))
+
+    def msckf_prepare_landmarks(self, batch, lm_featid, lm_planeid, sigma_pix=1.0, chi2_mult=1.0):
+        fb, keep = self._batch_struct(batch)
+        lm, keep_lm = self._landmarks_struct(lm_featid, lm_planeid)
+        self._prep_F, self._prep_np = fb.F, fb.nplanes
+        uo = UpdaterOptions(sigma_pix, chi2_mult)
+        self._ck(self.lib.ovp_msckf_prepare_landmarks(self.h, C.byref(fb), C.byref(lm), C.byref(uo)))
 
     def msckf_launch(self):
         self._ck(self.lib.ovp_msckf_launch(self.h))

@@ -781,12 +781,24 @@ int ovp_plane_measurement_compress_inplace(ovp_ctx *h, double *H_x, int cols, do
 }
 
 // ---- UpdaterMSCKF ------------------------------------------------------------------------------------------------------
-int ovp_msckf_update(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updater_options *opt, int *feat_status, double *feat_chi2,
-                     int *plane_status, double *plane_chi2, int *hx_order, int *hx_order_n) {
+// an empty landmark list is the plain update (same plan, same signature)
+static const MsckfExtra *landmark_extra(const ovp_plane_landmarks *lm, MsckfExtra &ex) {
+  if (!lm || lm->n == 0)
+    return nullptr;
+  ex.landmarks = lm;
+  return &ex;
+}
+int ovp_msckf_update_landmarks(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_plane_landmarks *landmarks, const ovp_updater_options *opt,
+                               int *feat_status, double *feat_chi2, int *plane_status, double *plane_chi2, int *hx_order, int *hx_order_n) {
   Ctx *c = ovp::enter(h);
   if (!batch || !opt)
     return fail(c, OVP_ERR_BAD_ARGS, "null batch / options");
-  return msckf_update_impl(c, batch, opt, feat_status, feat_chi2, plane_status, plane_chi2, hx_order, hx_order_n, nullptr);
+  MsckfExtra ex;
+  return msckf_update_impl(c, batch, opt, feat_status, feat_chi2, plane_status, plane_chi2, hx_order, hx_order_n, landmark_extra(landmarks, ex));
+}
+int ovp_msckf_update(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updater_options *opt, int *feat_status, double *feat_chi2,
+                     int *plane_status, double *plane_chi2, int *hx_order, int *hx_order_n) {
+  return ovp_msckf_update_landmarks(h, batch, nullptr, opt, feat_status, feat_chi2, plane_status, plane_chi2, hx_order, hx_order_n);
 }
 
 static int shard_cols(Ctx *c, const int *all_clone_handles, int n_clones, std::vector<int> &cols) {
@@ -1353,11 +1365,15 @@ int ovp_selftest_dgemm_tflops(ovp_ctx *h, int n, int iters, double *tflops) {
 // ---- prepared-batch variant of UpdaterMSCKF::update, snapshots and per-kernel profiling (measurement support) ----------
 extern "C" {
 
-int ovp_msckf_prepare(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updater_options *opt) {
+int ovp_msckf_prepare_landmarks(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_plane_landmarks *landmarks, const ovp_updater_options *opt) {
   Ctx *c = ovp::enter(h);
   if (!batch || !opt)
     return fail(c, OVP_ERR_BAD_ARGS, "null batch / options");
-  return msckf_prepare(c, batch, opt, nullptr);
+  MsckfExtra ex;
+  return msckf_prepare(c, batch, opt, landmark_extra(landmarks, ex));
+}
+int ovp_msckf_prepare(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updater_options *opt) {
+  return ovp_msckf_prepare_landmarks(h, batch, nullptr, opt);
 }
 int ovp_msckf_launch(ovp_ctx *h) { return msckf_launch(&h->c); }
 int ovp_msckf_finish(ovp_ctx *h, int *feat_status, double *feat_chi2, int *plane_status, double *plane_chi2, int *hx_order, int *hx_order_n) {

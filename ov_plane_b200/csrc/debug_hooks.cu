@@ -281,12 +281,16 @@ extern "C" int ovp_debug_chol_products(ovp_ctx *h, const double *G, int nc, int 
 // feature kernel.  raw_out (optional, 3 * OVP_RAW_ROW doubles per measurement, OVP_RAW_ROW in features.cu): the raw whitened rows the
 // feature kernel built.  A plan that goes straight into the update (no compression) has no Gram matrix: OVP_ERR_BAD_ARGS.  Not part of
 // the ABI in include/ovp.h.
-extern "C" int ovp_debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, const ovp_updater_options *opt, int gcap, double *G_out,
-                                    int *info, int *cols_out, int *sel_out, int *feat_status, double *feat_chi2, double *raw_out) {
+// ovp_debug_msckf_gram_landmarks: the same with the landmark members of ovp_msckf_update_landmarks (their columns follow the x columns
+// of the batch features, ncx counts them).
+static int debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, const ovp_plane_landmarks *lm, const ovp_updater_options *opt, int gcap,
+                            double *G_out, int *info, int *cols_out, int *sel_out, int *feat_status, double *feat_chi2, double *raw_out) {
   Ctx *c = ovp::enter(h);
   if (!b || !opt || b->F <= 0)
     return fail(c, OVP_ERR_BAD_ARGS, "debug_msckf_gram: empty batch");
-  int st = msckf_prepare(c, b, opt, nullptr);
+  MsckfExtra ex;
+  ex.landmarks = lm;
+  int st = msckf_prepare(c, b, opt, lm && lm->n > 0 ? &ex : nullptr);
   if (st)
     return st;
   Prepared &P = *(Prepared *)c->prep;
@@ -310,13 +314,16 @@ extern "C" int ovp_debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, cons
     if (c->dbg_gram_plan < 0)
       return fail(c, OVP_ERR_BAD_ARGS, "debug_msckf_gram: the first plan goes straight into the update, without a Gram matrix");
     const UpdatePlan &pl = P.plans[c->dbg_gram_plan];
-    const int ncx = (int)pl.cols.size(), nc1 = pl.is_point ? ncx + 1 : ncx + 4;
+    const int ncx = pl.nx(), nc1 = pl.is_point ? ncx + 1 : ncx + 4;
     if (nc1 > gcap)
       return fail(c, OVP_ERR_CAPACITY, "debug_msckf_gram: %d columns, room for %d", nc1, gcap);
     const int ncal = (c->opt.do_calib_camera_pose ? 6 : 0) + (c->opt.do_calib_camera_intrinsics ? 8 : 0);
     const int v[8] = {nc1, ncal, ncx, pl.is_point ? 1 : 0, (int)pl.feats.size(), P.fast ? 1 : 0, pl.plane_slot, pl.in_state ? 1 : 0};
     std::memcpy(info, v, sizeof(v));
-    std::memcpy(cols_out, pl.cols.data(), ncx * sizeof(int));
+    std::memcpy(cols_out, pl.cols.data(), pl.cols.size() * sizeof(int));
+    for (size_t k = 0; k < pl.lm_handle.size(); k++)
+      for (int j = 0; j < 3; j++)
+        cols_out[pl.cols.size() + 3 * k + j] = c->vars[pl.lm_handle[k]].id + j;
     std::memcpy(sel_out, pl.feats.data(), pl.feats.size() * sizeof(int));
     OVP_CUDA(cudaMemcpy2DAsync(G_out, (size_t)nc1 * sizeof(double), c->wsG.S, (size_t)c->wsG.cap * sizeof(double), (size_t)nc1 * sizeof(double),
                                nc1, cudaMemcpyDeviceToHost, c->stream));
@@ -335,4 +342,13 @@ extern "C" int ovp_debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, cons
   if (draw)
     cudaFree(draw);
   return st;
+}
+extern "C" int ovp_debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, const ovp_updater_options *opt, int gcap, double *G_out,
+                                    int *info, int *cols_out, int *sel_out, int *feat_status, double *feat_chi2, double *raw_out) {
+  return debug_msckf_gram(h, b, nullptr, opt, gcap, G_out, info, cols_out, sel_out, feat_status, feat_chi2, raw_out);
+}
+extern "C" int ovp_debug_msckf_gram_landmarks(ovp_ctx *h, const ovp_feature_batch *b, const ovp_plane_landmarks *lm, const ovp_updater_options *opt,
+                                              int gcap, double *G_out, int *info, int *cols_out, int *sel_out, int *feat_status, double *feat_chi2,
+                                              double *raw_out) {
+  return debug_msckf_gram(h, b, lm, opt, gcap, G_out, info, cols_out, sel_out, feat_status, feat_chi2, raw_out);
 }

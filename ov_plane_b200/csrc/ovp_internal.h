@@ -234,6 +234,7 @@ struct MsckfExtra {
                                // in rank order on every rank, then the ordinary compression + EKF update (replicated)
   int64_t only_plane_id = 0;   // init_vio_plane: build the W system of this (out-of-state) plane only and stop
   double sigma_c_scale = 0.0;  // > 0: multiply sigma_constraint (const_init_multi)
+  const ovp_plane_landmarks *landmarks = nullptr; // use_plane_constraint_slamu: candidate landmark members of the out-of-state planes
 };
 int msckf_last_W(Ctx *c, int *rowsW, int *ncx, int *rows_ref, const int **d_cols);
 int allgather_gram(Ctx *c, int nc1); // capi_nccl.inc: wsG.S (rank-local Gram, lower) -> sum over the ranks of the ctx's communicator
