@@ -16,6 +16,9 @@ struct StateOptions {
   double sigma_constraint = 0.01;
   int plane_msckf_min_feat = 20;
   double plane_msckf_max_cond = 100.0;
+  int max_msckf_plane = 20; // StateOptions.h: per-plane feature cap of init_vio_plane
+  int plane_init_min_feat = 8;
+  double plane_init_max_cond = 200.0;
 };
 class State {
 public:

@@ -336,6 +336,47 @@ int ovp_optimize_plane(ovp_ctx *ctx, int n_planes, const int *feat_offset, const
                        const double *p_FinG, const double *cp_inG, const int *fix_plane, const ovp_plane_refine_options *opt, double *p_FinG_out,
                        double *cp_out, int *inlier, int *status, double *info);
 
+/* ---- UpdaterPlane::init_vio_plane end to end (UpdaterPlane.cpp:61-481): new planes from raw feature tracks ------------------------------ */
+/* The caller's Feature objects after clean_old_measurements against the clone times, flattened: measurements in time order, clone handles,
+ * raw pixels (for the Jacobians) and undistorted normalised coordinates (for triangulation and refinement). */
+typedef struct ovp_feature_tracks {
+  int F;
+  const int *meas_offset; /* F+1 prefix offsets into the measurement arrays */
+  const int *meas_clone;  /* clone handle per measurement */
+  const float *uv;        /* Feature::uvs (raw pixels), 2 per measurement */
+  const float *uv_norm;   /* Feature::uvs_norm, 2 per measurement */
+  const int64_t *featid;  /* F, distinct */
+  const int64_t *planeid; /* F: feat2plane entry, 0 = none */
+} ovp_feature_tracks;
+typedef struct ovp_plane_init_options {
+  double sigma_pix;                     /* UpdaterOptions::sigma_pix of the MSCKF updater */
+  int max_msckf_plane;                  /* StateOptions: a plane keeps its max_msckf_plane + 1 shortest tracks (UpdaterPlane.cpp:189) */
+  int plane_init_min_feat;              /* StateOptions: RANSAC's inlier minimum */
+  double plane_init_max_cond;           /* StateOptions: RANSAC's condition-number limit */
+  int shuffle_kind;                     /* as ovp_plane_fit_options */
+  const ovp_triangulation_options *tri; /* NULL = OpenVINS defaults */
+} ovp_plane_init_options;
+/* Candidates are the features on a plane that is not in the state; those with fewer than two measurements are dropped, the others are
+ * triangulated, sorted by track length with std::sort (ascending, not stable), grouped per plane under the cap, fitted by RANSAC
+ * (plane_init_min_feat / plane_init_max_cond) and refined jointly with the plane free (sigma_pix / fx of the current intrinsics,
+ * sigma_constraint); every plane that obtained a linearisation point is then initialised like ovp_plane_init, ascending id.
+ * The measurements cross to the device once; between stages only statuses, inlier flags and the refined plane come back.
+ * feat_status[F]: -1 fewer than 2 measurements (erase it from feature_vec), -2 triangulation failed (keep it), 0 not a candidate,
+ * 2 candidate not consumed, 1 consumed by an initialised plane (to_delete, moved to feature_vec_used).
+ * p_FinG_out[3F]: triangulated position (for -2, whatever the failed triangulation produced, as the reference leaves it in the Feature), or
+ * the refinement's output for the features that went into a refinement; zero for features with status 0 or -1.  Plane outputs, sized F entries by the caller (at most one plane per feature): *n_planes planes, every plane
+ * with a candidate after triangulation, ascending id; plane_status 1 initialised, 0 rejected by initialize's chi2, -2 RANSAC returned false,
+ * -3 optimize_plane returned false, -1 not attempted (fewer than 3 features left); new_handles (or -1); cp_out[3 * n_planes] the
+ * linearisation point handed to initialize (the refinement's plane, zero when RANSAC failed).
+ * Refused before anything is copied or launched, with the state untouched: a null pointer, meas_offset not starting at 0 or decreasing, a
+ * duplicate featid, a candidate measurement whose handle is not a clone (or that observes a clone twice), OVP_ERR_CAPACITY for a candidate
+ * track longer than the plane-system limit (37, see ovp_msckf_update) or max_msckf_plane + 1 above RANSAC's 1900 points.  The capacities of
+ * the initialisation stage itself (rows of one plane's stacked system against max_meas_rows, three more state rows per new plane against
+ * max_state) depend on RANSAC's and the refinement's outcome and are checked by that stage as in ovp_plane_init: such a refusal comes after
+ * the plane-fitting launches, leaves the plane it concerns (and the later ones) uninitialised, and keeps the planes initialised before it. */
+int ovp_plane_init_tracks(ovp_ctx *ctx, const ovp_feature_tracks *t, const ovp_plane_init_options *opt, int *feat_status, double *p_FinG_out,
+                          int *n_planes, int64_t *plane_ids, int *plane_status, int *new_handles, double *cp_out);
+
 /* ---- UpdaterZeroVelocity (update/UpdaterZeroVelocity.cpp:68-318) ------------------------------------------------------- */
 typedef struct ovp_zupt_options {
   double gravity_mag;           /* VioManagerOptions.h:206 */

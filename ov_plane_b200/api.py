@@ -50,6 +50,16 @@ class PlaneRefineOptions(C.Structure):
     _fields_ = [("sigma_px_norm", C.c_double), ("sigma_c", C.c_double), ("max_num_iterations", C.c_int)]
 
 
+class FeatureTracks(C.Structure):
+    _fields_ = [("F", C.c_int), ("meas_offset", C.c_void_p), ("meas_clone", C.c_void_p), ("uv", C.c_void_p), ("uv_norm", C.c_void_p),
+                ("featid", C.c_void_p), ("planeid", C.c_void_p)]
+
+
+class PlaneInitOptions(C.Structure):
+    _fields_ = [("sigma_pix", C.c_double), ("max_msckf_plane", C.c_int), ("plane_init_min_feat", C.c_int), ("plane_init_max_cond", C.c_double),
+                ("shuffle_kind", C.c_int), ("tri", C.c_void_p)]
+
+
 DEBUG_LIB_PATH = os.path.join(_HERE, "lib", "libovp_debug.so")  # product sources + include/ovp_debug.h hooks (tools/, kernel unit tests)
 
 
@@ -404,6 +414,24 @@ class Context(object):
         ps, nh = np.zeros(npl, dtype=np.int32), np.zeros(npl, dtype=np.int32)
         self._ck(self.lib.ovp_plane_init(self.h, C.byref(fb), C.byref(uo), _p(ps), _p(nh)))
         return dict(plane_status=ps[:fb.nplanes], new_handles=nh[:fb.nplanes])
+
+    def plane_init_tracks(self, tracks, sigma_pix=1.0, max_msckf_plane=20, plane_init_min_feat=8, plane_init_max_cond=200.0, shuffle_kind=0):
+        """UpdaterPlane::init_vio_plane end to end on raw tracks (dict: meas_offset, meas_clone, uv, uv_norm, featid, planeid; see
+        include/ovp.h ovp_plane_init_tracks).  Returns feat_status, p_FinG, plane_ids, plane_status, new_handles, cp."""
+        mo, mc = _i32(tracks["meas_offset"]), _i32(tracks["meas_clone"])
+        uv = np.ascontiguousarray(tracks["uv"], dtype=np.float32)
+        uvn = np.ascontiguousarray(tracks["uv_norm"], dtype=np.float32)
+        fid = np.ascontiguousarray(tracks["featid"], dtype=np.int64)
+        pid = np.ascontiguousarray(tracks["planeid"], dtype=np.int64)
+        F = len(mo) - 1
+        t = FeatureTracks(F, mo.ctypes.data, mc.ctypes.data, uv.ctypes.data, uvn.ctypes.data, fid.ctypes.data, pid.ctypes.data)
+        o = PlaneInitOptions(float(sigma_pix), int(max_msckf_plane), int(plane_init_min_feat), float(plane_init_max_cond), int(shuffle_kind), None)
+        n = max(1, F)
+        fs, pf, npl = np.zeros(n, dtype=np.int32), np.zeros((n, 3)), C.c_int(0)
+        pids, ps, nh, cp = np.zeros(n, dtype=np.int64), np.zeros(n, dtype=np.int32), np.zeros(n, dtype=np.int32), np.zeros((n, 3))
+        self._ck(self.lib.ovp_plane_init_tracks(self.h, C.byref(t), C.byref(o), _p(fs), _p(pf), C.byref(npl), _p(pids), _p(ps), _p(nh), _p(cp)))
+        k = npl.value
+        return dict(feat_status=fs[:F], p_FinG=pf[:F], plane_ids=pids[:k], plane_status=ps[:k], new_handles=nh[:k], cp=cp[:k])
 
     # ---- UpdaterSLAM ----
     def slam_update(self, b, sigma_pix=1.0, chi2_mult=1.0, use_plane_constraint=True):

@@ -367,15 +367,15 @@ int ovp_initialize(ovp_ctx *h, int kind, int s, const double *value, const doubl
   return initialize_core(c, kind, s, value, fej, tag, c->dcols, n, W, rows, rows, rows, sigma2, chi2_mult, do_update, accepted, new_handle);
 }
 
+} // extern "C"
+
+namespace ovp {
 // UpdaterPlane::init_vio_plane from "plane linearisation points known" on (UpdaterPlane.cpp:297-481): for every plane of the
 // batch that is NOT in the state (ascending id, std::map order) and has >= 3 features: per-feature Jacobians with
 // sigma_c * const_init_multi (:384), H_cp split off H_f (:388-390), left-nullspace projection, stacking, compression and
 // StateHelper::initialize(plane Vec(3), ..., const_init_chi2) (:436-446).  plane_status[i]: 1 initialised, 0 chi2-rejected,
-// -1 not attempted; new_handles[i]: handle of the new plane variable or -1.
-int ovp_plane_init(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updater_options *opt, int *plane_status, int *new_handles) {
-  Ctx *c = ovp::enter(h);
-  if (!batch || !opt || !batch->plane_cp)
-    return fail(c, OVP_ERR_BAD_ARGS, "plane_init: null batch / options / plane_cp");
+// -1 not attempted; new_handles[i]: handle of the new plane variable or -1.  Shared by ovp_plane_init and ovp_plane_init_tracks.
+int plane_init_core(Ctx *c, const ovp_feature_batch *batch, const ovp_updater_options *opt, int *plane_status, int *new_handles) {
   std::vector<std::pair<int64_t, int>> ps;
   for (int i = 0; i < batch->nplanes; i++) {
     ps.push_back({batch->plane_ids[i], i});
@@ -420,6 +420,16 @@ int ovp_plane_init(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updater
     new_handles[pp.second] = nh;
   }
   return OVP_OK;
+}
+} // namespace ovp
+
+extern "C" {
+
+int ovp_plane_init(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updater_options *opt, int *plane_status, int *new_handles) {
+  Ctx *c = ovp::enter(h);
+  if (!batch || !opt || !batch->plane_cp)
+    return fail(c, OVP_ERR_BAD_ARGS, "plane_init: null batch / options / plane_cp");
+  return ovp::plane_init_core(c, batch, opt, plane_status, new_handles);
 }
 
 int ovp_merge_planes_and_marginalize(ovp_ctx *h, const int64_t *f2p_feat, const int64_t *f2p_plane, int nf, const int64_t *merge_new,
