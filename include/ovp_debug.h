@@ -4,8 +4,10 @@
  * product library libovp.so does not export them.  They let tools/microbench_chol.py time the fused Cholesky, let
  * tests/test_gpu_cholfused.py / tests/test_gpu_gemm.py / tests/test_gpu_gemm_split.py unit-test chol_fused_kernel and the DMMA GEMM against NumPy on arbitrary
  * matrices, let tests/test_gpu_numerics.py run one batch through both MSCKF feature paths, let tests/test_gpu_fused_products.py check the
- * update products formed inside the Gram factorisation and run the update both with and without them, and let
- * tests/test_gpu_compression.py check the compressed update's Gram matrix, zero-pivot rule and innovation gate element by element. */
+ * update products formed inside the Gram factorisation and run the update both with and without them, let
+ * tests/test_gpu_compression.py check the compressed update's Gram matrix, zero-pivot rule and innovation gate element by element, and
+ * let tests/test_gpu_feature_gate.py check the per-feature chi2 gates of the MSCKF point and SLAM feature kernels against long-double
+ * references on the raw rows those kernels built. */
 #ifndef OVP_DEBUG_H
 #define OVP_DEBUG_H
 #include "ovp.h"
@@ -67,6 +69,12 @@ int ovp_debug_msckf_gram(ovp_ctx *ctx, const ovp_feature_batch *b, const ovp_upd
 int ovp_debug_msckf_gram_landmarks(ovp_ctx *ctx, const ovp_feature_batch *b, const ovp_plane_landmarks *lm, const ovp_updater_options *opt,
                                    int gcap, double *G_out, int *info, int *cols_out, int *sel_out, int *feat_status, double *feat_chi2,
                                    double *raw_out);
+/* ovp_slam_update, which also returns the raw whitened rows the SLAM feature kernel built (tests/test_gpu_feature_gate.py): raw_out (NULL,
+ * or 72 doubles per measurement of the batch) in the layout of ovp_debug_msckf_gram, with [0,3) holding the landmark's columns in the
+ * bearing rows and in the point-on-plane row.  The update runs as ovp_slam_update runs it. */
+int ovp_debug_slam_update(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
+                          const int64_t *planeid, const ovp_updater_options *opt, int use_plane_constraint, int *feat_status, double *feat_chi2,
+                          double *raw_out);
 
 #ifdef __cplusplus
 }

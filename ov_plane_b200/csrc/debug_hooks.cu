@@ -2,7 +2,8 @@
 // Declared in include/ovp_debug.h.  Used by tools/microbench_chol.py (phase timeline of the fused Cholesky), by
 // tests/test_gpu_cholfused.py and tests/test_gpu_gemm.py (unit tests of chol_fused_kernel and the DMMA GEMM against NumPy), by
 // tests/test_gpu_numerics.py (the block-sparse feature path against the dense stack on the same batch) and by tests/test_gpu_compression.py
-// (the compressed update's Gram matrix, zero-pivot rule and innovation gate against long-double references).
+// (the compressed update's Gram matrix, zero-pivot rule and innovation gate against long-double references) and by
+// tests/test_gpu_feature_gate.py (the per-feature chi2 gates of the MSCKF point and SLAM feature kernels).
 #include "ovp_internal.h"
 using namespace ovp;
 
@@ -351,4 +352,35 @@ extern "C" int ovp_debug_msckf_gram_landmarks(ovp_ctx *h, const ovp_feature_batc
                                               int gcap, double *G_out, int *info, int *cols_out, int *sel_out, int *feat_status, double *feat_chi2,
                                               double *raw_out) {
   return debug_msckf_gram(h, b, lm, opt, gcap, G_out, info, cols_out, sel_out, feat_status, feat_chi2, raw_out);
+}
+
+// Test hook (tests/test_gpu_feature_gate.py): ovp_slam_update, which also returns the raw whitened rows the SLAM feature kernel built
+// (raw_out: 3 * OVP_RAW_ROW doubles per measurement of the batch, OVP_RAW_ROW in features.cu, [0,3) holding the landmark's columns).  The
+// update itself runs as ovp_slam_update runs it.  Not part of the ABI in include/ovp.h.
+extern "C" int ovp_debug_slam_update(ovp_ctx *h, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
+                                     const int64_t *planeid, const ovp_updater_options *opt, int use_plane_constraint, int *feat_status,
+                                     double *feat_chi2, double *raw_out) {
+  Ctx *c = ovp::enter(h);
+  if (F > 0 && (!meas_offset || !meas_clone || !uv || !featid || !opt))
+    return fail(c, OVP_ERR_BAD_ARGS, "debug_slam_update: null argument");
+  const size_t nraw = (size_t)3 * OVP_RAW_ROW * std::max(F > 0 ? meas_offset[F] : 0, 1);
+  double *draw = nullptr;
+  if (raw_out) {
+    OVP_CUDA(cudaMalloc(&draw, nraw * sizeof(double)));
+    OVP_CUDA(cudaMemsetAsync(draw, 0, nraw * sizeof(double), c->stream));
+  }
+  c->dbg_raw = draw;
+  int st = slam_update_impl(c, F, meas_offset, meas_clone, uv, featid, planeid, opt, use_plane_constraint, feat_status, feat_chi2);
+  c->dbg_raw = nullptr;
+  auto run = [&]() -> int {
+    if (st || !raw_out)
+      return st;
+    OVP_CUDA(cudaMemcpyAsync(raw_out, draw, nraw * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaStreamSynchronize(c->stream));
+    return OVP_OK;
+  };
+  st = run();
+  if (draw)
+    cudaFree(draw);
+  return st;
 }

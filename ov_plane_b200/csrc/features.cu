@@ -18,9 +18,10 @@
 namespace ovp {
 
 #ifdef OVP_DEBUG
-// Raw whitened blocks of the MSCKF feature kernels as they hold them (ovp_debug_msckf_gram, libovp_debug.so only).  Measurement g of the
-// batch owns 3 rows of OVP_RAW_ROW doubles from raw[g * 3 * OVP_RAW_ROW]: its two bearing rows, [0,3) H_f, [3,9) H_clone,
-// [9, 9 + ncal) calibration, [23] r; in plane mode its point-on-plane row, [0,3) H_f, [9,12) H_cp, [23] r.  Entries not named are left.
+// Raw whitened blocks of the feature kernels as they hold them (ovp_debug_msckf_gram, ovp_debug_slam_update; libovp_debug.so only).
+// Measurement g of the batch owns 3 rows of OVP_RAW_ROW doubles from raw[g * 3 * OVP_RAW_ROW]: its two bearing rows, [0,3) H_f (SLAM: the
+// landmark's columns), [3,9) H_clone, [9, 9 + ncal) calibration, [23] r; with a plane its point-on-plane row, [0,3) H_f, [9,12) H_cp,
+// [23] r.  Entries not named are left.
 #define OVP_RAW_ROW 24
 #endif
 struct FeatArgs {
@@ -238,7 +239,7 @@ __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
       A[(size_t)c_res * lda + r] = res[i];
     }
 #ifdef OVP_DEBUG
-    if (a.raw && a.mode != 2) // the rows just written to A, in the layout of OVP_RAW_ROW
+    if (a.raw) // the rows just written to A, in the layout of OVP_RAW_ROW (SLAM: [0,3) are the landmark's columns)
       for (int i = 0; i < 2; i++) {
         double *rw = a.raw + ((size_t)(m0 + k) * 3 + i) * OVP_RAW_ROW;
         for (int j = 0; j < 3 + cf; j++)
@@ -268,7 +269,7 @@ __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
       }
       A[(size_t)c_res * lda + r] = pr;
 #ifdef OVP_DEBUG
-      if (a.raw && a.mode == 1) {
+      if (a.raw) {
         double *rw = a.raw + ((size_t)(m0 + k) * 3 + 2) * OVP_RAW_ROW;
         for (int j = 0; j < 3; j++) {
           rw[j] = A[(size_t)j * lda + r];

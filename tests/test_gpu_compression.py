@@ -20,6 +20,7 @@ import pytest
 
 from conftest import make_pair
 from ov_plane_b200 import api, synth
+from gate_reference import householder_q3
 from test_gpu_parity import _check_msckf, oracle_msckf_update, relerr
 
 pytestmark = pytest.mark.gpu
@@ -46,10 +47,10 @@ def _require_long_double():
 # ---------------------------------------------------------------------------------------------------------------------------------
 # 1. Gram matrix
 # ---------------------------------------------------------------------------------------------------------------------------------
-def run_gram(ctx, batch, dense):
+def run_gram(ctx, batch, dense, sigma_pix=1.0, chi2_mult=1.0):
     """ovp_debug_msckf_gram on one batch: G, the plan's layout, statuses and the raw rows of every measurement."""
     fb, keep = api.Context._batch_struct(batch)
-    uo = api.UpdaterOptions(1.0, 1.0)
+    uo = api.UpdaterOptions(sigma_pix, chi2_mult)
     F, M = fb.F, int(batch["meas_offset"][-1])
     gcap = ctx.cov_rows() + 4
     G = np.zeros(gcap * gcap)
@@ -86,28 +87,6 @@ def feature_block(r, batch, f):
             X[2 * m + k, -4:-1] = row[9:12]
             X[2 * m + k, -1] = row[RAW_ROW - 1]
     return X
-
-
-def householder_q3(Hf):
-    """First three columns of Q of Hf = Q R (3 Householder reflectors, long double)."""
-    A = Hf.copy()
-    n = A.shape[0]
-    vs = []
-    for j in range(3):
-        x = A[j:, j].copy()
-        nrm = np.sqrt((x * x).sum())
-        alpha = -nrm if x[0] > 0 else nrm
-        v = x.copy()
-        v[0] -= alpha
-        vtv = (v * v).sum()
-        beta = 2 / vtv if vtv > 0 else LD(0)
-        A[j:, :] -= beta * np.outer(v, v @ A[j:, :])
-        vs.append((j, v, beta))
-    Q = np.zeros((n, 3), dtype=LD)
-    Q[:3, :3] = np.eye(3, dtype=LD)
-    for j, v, beta in reversed(vs):
-        Q[j:, :] -= beta * np.outer(v, v @ Q[j:, :])
-    return Q
 
 
 def gram_reference(r, batch, var_id):
