@@ -140,7 +140,8 @@ int ovp_feature_jacobian_full(ovp_ctx *ctx, int m, const int *clone_handles, con
                               int *x_order, int *x_order_n);
 /* UpdaterHelper::nullspace_project_inplace (:515-546) / UpdaterPlane::nullspace_project_inplace (UpdaterPlane.cpp:483-517).
  * Result is an orthogonal-equivalent left-nullspace projection (Householder instead of the reference's Givens order):
- * identical H_o^T H_o, H_o^T r and chi2; rows of H_o differ by an orthogonal transform (SURVEY §7 hazard list). */
+ * identical H_o^T H_o, H_o^T r and chi2; rows of H_o differ by an orthogonal transform (SURVEY §7 hazard list).
+ * Any rows >= hf_cols are projected (rows == hf_cols returns *rows_out = 0); an exactly zero column of H_f is skipped. */
 int ovp_nullspace_project_inplace(ovp_ctx *ctx, double *H_f, int hf_cols, double *H_x, int hx_cols, double *res, int rows,
                                   int *rows_out);
 int ovp_plane_nullspace_project_inplace(ovp_ctx *ctx, double *H_f, int hf_cols, double *H_x, int hx_cols, double *H_cp,

@@ -98,8 +98,10 @@ __global__ void init_grow_kernel(double *P, int ld, int N, int s, const double *
       v = 0.0;
       for (int k = 0; k < s; k++)
         v -= Ma[(size_t)k * ldm + i] * HLinv[(size_t)k * s + j]; // (-M_a * H_Linv^T)(i,j) = -sum_k M_a(i,k) H_Linv(j,k)
-    } else {
-      v = PLL[(size_t)j * s + (i - N)];
+    } else { // P_LL from its lower triangle: the host product H_Linv M H_Linv^T is symmetric to rounding only, and the threads of
+             // (r, j) and (j, r) both write both entries
+      const int r = i - N;
+      v = PLL[(size_t)min(r, j) * s + max(r, j)];
     }
     P[(size_t)(N + j) * ld + i] = v;
     P[(size_t)i * ld + (N + j)] = v;

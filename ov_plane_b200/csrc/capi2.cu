@@ -310,8 +310,9 @@ int initialize_core(Ctx *c, int kind, int s, const double *value, const double *
     return fail(c, OVP_ERR_BAD_ARGS, "initialize: chi2 table too short for %d rows", dof_rows);
   if (rows - s > c->Rcap)
     return fail(c, OVP_ERR_CAPACITY, "initialize: %d rows exceed capacity", rows);
-  householder_cols_kernel<<<1, 256, (size_t)rows * sizeof(double), c->stream>>>(W, ldW, rows, s + n + 1, s);
+  householder_cols_kernel<<<1, 256, 0, c->stream>>>(W, ldW, rows, s + n + 1, s);
   c->launches++;
+  OVP_CUDA(cudaGetLastError());
   const int ru = rows - s;
   double *dR = c->dvec + 3 * (size_t)c->Rcap;
   MatView HupT = mv(W + (size_t)s * ldW + s, ldW, 1);
@@ -719,16 +720,20 @@ static int nullspace_common(Ctx *c, double *H_f, int hf_cols, double *H_x, int h
   if (H_cp)
     OVP_CUDA(cudaMemcpyAsync(W + (size_t)rows * (hf_cols + hx_cols), H_cp, (size_t)rows * 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   OVP_CUDA(cudaMemcpyAsync(W + (size_t)rows * (hf_cols + hx_cols + ncp), res, (size_t)rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  householder_cols_kernel<<<1, 256, (size_t)rows * sizeof(double), c->stream>>>(W, rows, rows, ncols, hf_cols);
+  householder_cols_kernel<<<1, 256, 0, c->stream>>>(W, rows, rows, ncols, hf_cols);
   c->launches++;
+  OVP_CUDA(cudaGetLastError());
   int ro = rows - hf_cols;
-  // copy back rows [hf_cols, rows) compacted to ld = ro
-  OVP_CUDA(cudaMemcpy2DAsync(H_x, (size_t)ro * sizeof(double), W + (size_t)rows * hf_cols + hf_cols, (size_t)rows * sizeof(double),
-                             (size_t)ro * sizeof(double), hx_cols, cudaMemcpyDeviceToHost, c->stream));
-  if (H_cp)
-    OVP_CUDA(cudaMemcpy2DAsync(H_cp, (size_t)ro * sizeof(double), W + (size_t)rows * (hf_cols + hx_cols) + hf_cols, (size_t)rows * sizeof(double),
-                               (size_t)ro * sizeof(double), 3, cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(res, W + (size_t)rows * (hf_cols + hx_cols + ncp) + hf_cols, (size_t)ro * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  // copy back rows [hf_cols, rows) compacted to ld = ro (none when H_f is square)
+  if (ro > 0) {
+    OVP_CUDA(cudaMemcpy2DAsync(H_x, (size_t)ro * sizeof(double), W + (size_t)rows * hf_cols + hf_cols, (size_t)rows * sizeof(double),
+                               (size_t)ro * sizeof(double), hx_cols, cudaMemcpyDeviceToHost, c->stream));
+    if (H_cp)
+      OVP_CUDA(cudaMemcpy2DAsync(H_cp, (size_t)ro * sizeof(double), W + (size_t)rows * (hf_cols + hx_cols) + hf_cols,
+                                 (size_t)rows * sizeof(double), (size_t)ro * sizeof(double), 3, cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaMemcpyAsync(res, W + (size_t)rows * (hf_cols + hx_cols + ncp) + hf_cols, (size_t)ro * sizeof(double), cudaMemcpyDeviceToHost,
+                             c->stream));
+  }
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   *rows_out = ro;
   return OVP_OK;

@@ -189,46 +189,50 @@ int chol_partial(Ctx *c, double *A, int ld, int n, int npiv, double tol) {
 }
 
 // stand-alone Householder left-nullspace projection on a global-memory matrix (col-major, ld): reflectors from the first
-// nref columns applied to all ncols columns.  One CTA.
+// nref columns applied to all ncols columns.  One CTA, any number of rows: the reflector v = [v0; A(j+1:, j)] is read from
+// column j itself (only v0 is kept in shared memory), and column j becomes [alpha; 0] once every trailing column has been reflected.
 __global__ void __launch_bounds__(256) householder_cols_kernel(double *A, int ld, int rows, int ncols, int nref) {
-  extern __shared__ double vbuf[];
-  __shared__ double s_beta;
+  __shared__ double s_v0, s_beta;
   const int tid = threadIdx.x;
   for (int j = 0; j < nref; j++) {
+    double *vcol = A + (size_t)j * ld;
+    double alpha = 0.0, nrm = 0.0;
     if (tid < 32) {
       double s = 0.0;
       for (int i = j + tid; i < rows; i += 32) {
-        double v = A[(size_t)j * ld + i];
+        double v = vcol[i];
         s += v * v;
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1)
         s += __shfl_xor_sync(0xffffffffu, s, o);
-      double x0 = A[(size_t)j * ld + j];
-      double nrm = sqrt(s);
-      double alpha = (x0 > 0.0) ? -nrm : nrm;
+      double x0 = vcol[j];
+      nrm = sqrt(s);
+      alpha = (x0 > 0.0) ? -nrm : nrm;
       double v0 = x0 - alpha;
       double vtv = s - x0 * x0 + v0 * v0;
-      for (int i = j + tid; i < rows; i += 32) {
-        vbuf[i] = (i == j) ? v0 : A[(size_t)j * ld + i];
-        if (nrm > 0.0)
-          A[(size_t)j * ld + i] = (i == j) ? alpha : 0.0; // the reflected column itself: [alpha; 0]
-      }
-      if (tid == 0)
+      if (tid == 0) {
+        s_v0 = v0;
         s_beta = (vtv > 0.0 && nrm > 0.0) ? 2.0 / vtv : 0.0;
+      }
     }
     __syncthreads();
-    const double beta = s_beta;
+    const double beta = s_beta, v0 = s_v0;
     for (int cidx = j + 1 + tid; cidx < ncols; cidx += 256) {
       double *col = A + (size_t)cidx * ld;
       double s = 0.0;
-      for (int i = j; i < rows; i++)
-        s += vbuf[i] * col[i];
+      s += v0 * col[j];
+      for (int i = j + 1; i < rows; i++)
+        s += vcol[i] * col[i];
       s *= beta;
-      for (int i = j; i < rows; i++)
-        col[i] -= s * vbuf[i];
+      col[j] -= s * v0;
+      for (int i = j + 1; i < rows; i++)
+        col[i] -= s * vcol[i];
     }
-    __syncthreads();
+    __syncthreads(); // every trailing column has read v: the reflected column itself becomes [alpha; 0]
+    if (tid < 32 && nrm > 0.0)
+      for (int i = j + tid; i < rows; i += 32)
+        vcol[i] = (i == j) ? alpha : 0.0;
   }
 }
 
