@@ -15,6 +15,8 @@ namespace ovp {
 // -------------------------------------------------------------------------------------------------------------------
 // small state kernels
 // -------------------------------------------------------------------------------------------------------------------
+// StateHelper::marginalize (StateHelper.cpp:302-318): x1x1, x1x2 and x2x2 are copied; x2x1 is the transpose of the new x1x2 block
+// (:311), not the stored x2x1, which differs from it wherever P is not exactly symmetric (EKFPropagation leaves it so, :103-105)
 __global__ void marginalize_copy_kernel(const double *src, double *dst, int ld, int N, int mid, int ms) {
   int Nn = N - ms;
   size_t total = (size_t)Nn * Nn;
@@ -22,18 +24,21 @@ __global__ void marginalize_copy_kernel(const double *src, double *dst, int ld, 
     int i = (int)(idx % Nn), j = (int)(idx / Nn);
     int si = i < mid ? i : i + ms;
     int sj = j < mid ? j : j + ms;
-    dst[(size_t)j * ld + i] = src[(size_t)sj * ld + si];
+    const bool x2x1 = i >= mid && j < mid;
+    dst[(size_t)j * ld + i] = x2x1 ? src[(size_t)si * ld + sj] : src[(size_t)sj * ld + si];
   }
 }
-// append a copy of the rows / cols of [old, old+s) at [N, N+s)   (StateHelper::clone, StateHelper.cpp:376-378)
+// append a copy of the rows / cols of [old, old+s) at [N, N+s)   (StateHelper::clone, StateHelper.cpp:376-378): the new x new block
+// from the old x old block, the column block from the old columns, the row block from the old rows.  Thread (i, j) writes P(i, N+j)
+// and, for i < N, P(N+j, i): every entry has one writer, and every read is of the first N rows and columns, which nothing writes.
 __global__ void clone_kernel(double *P, int ld, int N, int old, int s) {
   int total = (N + s) * s;
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
     int i = idx % (N + s), j = idx / (N + s);
     int si = i < N ? i : old + (i - N);
-    double v = P[(size_t)(old + j) * ld + si];
-    P[(size_t)(N + j) * ld + i] = v;
-    P[(size_t)i * ld + (N + j)] = v;
+    P[(size_t)(N + j) * ld + i] = P[(size_t)(old + j) * ld + si];
+    if (i < N)
+      P[(size_t)i * ld + (N + j)] = P[(size_t)i * ld + (old + j)];
   }
 }
 // augment_clone time-offset terms (StateHelper.cpp:613-624), two passes (the second reads the updated dt row)
