@@ -95,7 +95,6 @@ static void inverse3(const double *A, double *Ai) { // column-major 3x3, Gauss-J
       Ai[3 * j + i] = M[i][3 + j];
 }
 static bool is_relative(int rep) { return rep >= 2 && rep <= 5; }
-static bool is_clone(Ctx *c, int h) { return h >= 0 && h < (int)c->vars.size() && c->vars[h].alive && c->vars[h].kind == OVP_KIND_POSE && c->vars[h].id >= 0 && h != c->h_calib; }
 
 } // namespace ovp
 
@@ -109,7 +108,7 @@ int ovp_feature_jacobian_full_rep(ovp_ctx *h, int m, const int *clone_handles, c
   if (representation < 0 || representation > 5 || !p_F || !p_F_fej || !H_f || !H_x || !res)
     return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full_rep: bad representation / null argument");
   const bool rel = is_relative(representation);
-  if (rel && !is_clone(c, anchor_clone_handle))
+  if (rel && !is_clone(c, anchor_clone_handle, true))
     return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full_rep: anchor handle %d is not a clone in the state", anchor_clone_handle);
   int st = sync_host_values(c);
   if (st)
@@ -187,7 +186,7 @@ int ovp_slam_set_representation(ovp_ctx *h, int64_t featid, int representation, 
   if (representation < 0 || representation > 4)
     return fail(c, OVP_ERR_BAD_ARGS, "slam_set_representation: representation %d (0..4; the single-depth form needs the bearing the landmark was "
                                      "initialised with and is not carried)", representation);
-  if (is_relative(representation) && !is_clone(c, anchor_clone_handle))
+  if (is_relative(representation) && !is_clone(c, anchor_clone_handle, true))
     return fail(c, OVP_ERR_BAD_ARGS, "slam_set_representation: anchor handle %d is not a clone in the state", anchor_clone_handle);
   c->vars[it->second].rep = representation;
   c->vars[it->second].anchor = is_relative(representation) ? anchor_clone_handle : -1;
@@ -216,7 +215,7 @@ int ovp_slam_perform_anchor_change(ovp_ctx *h, int64_t featid, int new_anchor_cl
   if (!is_relative(rep) || h_old < 0)
     return fail(c, OVP_ERR_BAD_ARGS, "perform_anchor_change: landmark %lld is not in an anchored representation (assert, UpdaterSLAM.cpp:710-711)",
                 (long long)featid);
-  if (!is_clone(c, h_old) || !is_clone(c, new_anchor_clone_handle))
+  if (!is_clone(c, h_old, true) || !is_clone(c, new_anchor_clone_handle, true))
     return fail(c, OVP_ERR_BAD_ARGS, "perform_anchor_change: old / new anchor is not a clone in the state");
   int st = sync_host_values(c);
   if (st)

@@ -3,7 +3,6 @@
 // (compiled as part of the unity build ovp_unity.cu, after capi.cu)
 #include <climits>
 #include "host_math.h"
-#include "triangulate_core.h"
 
 using namespace ovp;
 
@@ -1472,90 +1471,6 @@ int ovp_transfer_bytes(ovp_ctx *h, int64_t *h2d, int64_t *d2h) {
 }
 
 } // extern "C"
-
-// ---- FeatureInitializer::single_triangulation + single_gaussnewton on the device (triangulate_core.h) --------------------------------
-namespace ovp {
-// camera pose of every clone handle: R_GtoCi = R_ItoC R_GtoIi, p_CiinG = p_IiinG - R_GtoCi^T p_IinC (UpdaterMSCKF.cpp:122-140)
-__global__ void cam_pose_kernel(int nh, const int *var_kind, const int *var_id, const double *val, int h_calib, double *Rc, double *pc) {
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h >= nh || var_kind[h] != OVP_KIND_POSE || var_id[h] < 0 || h == h_calib)
-    return;
-  const double *v = val + (size_t)h * OVP_VAL_STRIDE, *cal = val + (size_t)h_calib * OVP_VAL_STRIDE;
-  double Ri[9], RC[9], R[9];
-  quat_to_rot(v, Ri);
-  quat_to_rot(cal, RC);
-  mat3_mul(RC, Ri, R);
-  for (int i = 0; i < 9; i++)
-    Rc[9 * (size_t)h + i] = R[i];
-  for (int i = 0; i < 3; i++)
-    pc[3 * (size_t)h + i] = v[4 + i] - (R[i] * cal[4] + R[3 + i] * cal[5] + R[6 + i] * cal[6]);
-}
-__global__ void triangulate_kernel(int F, const int *meas_offset, const int *meas_clone, const float *uvn, const double *Rc, const double *pc,
-                                   TriOptions o, double *p_FinG, int *status) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= F)
-    return;
-  const int m0 = meas_offset[f], m = meas_offset[f + 1] - m0;
-  double pf[3] = {0.0, 0.0, 0.0};
-  const int ok = (m >= 2) ? triangulate_feature(m, meas_clone + m0, Rc, pc, uvn + 2 * (size_t)m0, o, pf) : 0;
-  status[f] = ok;
-  for (int i = 0; i < 3; i++)
-    p_FinG[3 * (size_t)f + i] = pf[i];
-}
-} // namespace ovp
-extern "C" int ovp_triangulate_features(ovp_ctx *h, int F, const int *meas_offset, const int *meas_clone, const float *uv_norm,
-                                        const ovp_triangulation_options *opt, double *p_FinG, int *status) {
-  Ctx *c = ovp::enter(h);
-  if (F <= 0)
-    return OVP_OK;
-  if (!meas_offset || !meas_clone || !uv_norm || !p_FinG || !status)
-    return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: null argument");
-  const int M = meas_offset[F];
-  for (int k = 0; k < M; k++) {
-    const int hh = meas_clone[k];
-    if (hh < 0 || hh >= (int)c->vars.size() || !c->vars[hh].alive || c->vars[hh].kind != OVP_KIND_POSE || c->vars[hh].id < 0 || hh == c->h_calib)
-      return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: measurement %d: handle %d is not a clone in the state", k, hh);
-  }
-  if (c->var_table_dirty) {
-    int st = upload_var_table(c);
-    if (st)
-      return st;
-  }
-  TriOptions o = {5, 1e-3, 1e10, 1e-6, 1e-6, 10.0, 0.10, 60.0, 40.0, 10000.0}; // FeatureInitializerOptions defaults (ov_core)
-  if (opt) {
-    o.max_runs = opt->max_runs;
-    o.init_lamda = opt->init_lamda;
-    o.max_lamda = opt->max_lamda;
-    o.min_dx = opt->min_dx;
-    o.min_dcost = opt->min_dcost;
-    o.lam_mult = opt->lam_mult;
-    o.min_dist = opt->min_dist;
-    o.max_dist = opt->max_dist;
-    o.max_baseline = opt->max_baseline;
-    o.max_cond_number = opt->max_cond_number;
-  }
-  const int nh = (int)c->vars.size();
-  // staging: [offsets | clones | uvn] in, [p_FinG | status] out, camera pose table
-  const size_t b_off = 0, b_cl = b_off + (size_t)(F + 1) * 4, b_uv = (b_cl + (size_t)M * 4 + 7) & ~(size_t)7, b_pf = (b_uv + (size_t)M * 8 + 7) & ~(size_t)7;
-  const size_t b_st = b_pf + (size_t)F * 24, b_R = (b_st + (size_t)F * 4 + 7) & ~(size_t)7, b_p = b_R + (size_t)nh * 72, b_end = b_p + (size_t)nh * 24;
-  int st = ensure_stage(c, b_end / 8 + 8);
-  if (st)
-    return st;
-  char *d = (char *)c->d_stage;
-  OVP_CUDA(cudaMemcpyAsync(d + b_off, meas_offset, (size_t)(F + 1) * 4, cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(d + b_cl, meas_clone, (size_t)M * 4, cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(d + b_uv, uv_norm, (size_t)M * 8, cudaMemcpyHostToDevice, c->stream));
-  c->h2d_bytes += (int64_t)((F + 1) * 4 + M * 12);
-  cam_pose_kernel<<<(nh + 127) / 128, 128, 0, c->stream>>>(nh, c->d_var_kind, c->d_var_id, c->d_val, c->h_calib, (double *)(d + b_R), (double *)(d + b_p));
-  triangulate_kernel<<<(F + 63) / 64, 64, 0, c->stream>>>(F, (const int *)(d + b_off), (const int *)(d + b_cl), (const float *)(d + b_uv),
-                                                          (const double *)(d + b_R), (const double *)(d + b_p), o, (double *)(d + b_pf), (int *)(d + b_st));
-  c->launches += 2;
-  OVP_CUDA(cudaMemcpyAsync(p_FinG, d + b_pf, (size_t)F * 24, cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(status, d + b_st, (size_t)F * 4, cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaStreamSynchronize(c->stream));
-  c->d2h_bytes += (int64_t)F * 28;
-  return OVP_OK;
-}
 
 // ---- UpdaterZeroVelocity::try_update (update/UpdaterZeroVelocity.cpp:68-318) -------------------------------------------------------------
 // With the flags the reference hard-codes (:113-116): measurements w_true = 0, a_true = 0 for every IMU interval between the state time and

@@ -255,4 +255,21 @@ static inline Ctx *enter(ovp_ctx *h) {
     cudaSetDevice(h->c.device);
   return &h->c;
 }
+
+// h names a clone (State::_clones_IMU): a live pose other than the camera extrinsics, which with need_slot must also have covariance
+// columns.  A measurement's clone, an anchor and a shard's clone list are checked with this.
+static inline bool is_clone(const Ctx *c, int h, bool need_slot) {
+  return h >= 0 && h < (int)c->vars.size() && c->vars[h].alive && c->vars[h].kind == OVP_KIND_POSE && h != c->h_calib &&
+         (!need_slot || c->vars[h].id >= 0);
+}
+
+// bump allocator of a staging buffer: consecutive slices, each starting 16-byte aligned
+struct StageLayout {
+  size_t top = 0;
+  size_t take(size_t bytes) {
+    const size_t at = top;
+    top = (top + bytes + 15) & ~(size_t)15;
+    return at;
+  }
+};
 } // namespace ovp

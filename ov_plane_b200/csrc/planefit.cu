@@ -19,6 +19,7 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include "triangulate_core.h"
 
 namespace ovp {
 
@@ -1004,9 +1005,211 @@ static void pf_permutations_copy(int F, int kind, int *dst) {
   std::memcpy(dst, it->second.data(), it->second.size() * sizeof(int));
 }
 
+// ---- the stage launchers on device buffers: triangulation, RANSAC, refinement ------------------------------------------------------------
+// Shared by the single-stage entry points below and by ovp_plane_init_tracks (plane_init_tracks.inc), which chains them without returning
+// the intermediate positions to the host.  Each launcher counts its launches; outputs are slices of the caller's staging buffer d.
+
+// camera pose of every clone handle: R_GtoCi = R_ItoC R_GtoIi, p_CiinG = p_IiinG - R_GtoCi^T p_IinC (UpdaterMSCKF.cpp:122-140)
+__global__ void cam_pose_kernel(int nh, const int *var_kind, const int *var_id, const double *val, int h_calib, double *Rc, double *pc) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= nh || var_kind[h] != OVP_KIND_POSE || var_id[h] < 0 || h == h_calib)
+    return;
+  const double *v = val + (size_t)h * OVP_VAL_STRIDE, *cal = val + (size_t)h_calib * OVP_VAL_STRIDE;
+  double Ri[9], RC[9], R[9];
+  quat_to_rot(v, Ri);
+  quat_to_rot(cal, RC);
+  mat3_mul(RC, Ri, R);
+  for (int i = 0; i < 9; i++)
+    Rc[9 * (size_t)h + i] = R[i];
+  for (int i = 0; i < 3; i++)
+    pc[3 * (size_t)h + i] = v[4 + i] - (R[i] * cal[4] + R[3 + i] * cal[5] + R[6 + i] * cal[6]);
+}
+// FeatureInitializer::single_triangulation + single_gaussnewton on the device (triangulate_core.h), a thread per feature
+__global__ void triangulate_kernel(int F, const int *meas_offset, const int *meas_clone, const float *uvn, const double *Rc, const double *pc,
+                                   TriOptions o, double *p_FinG, int *status) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F)
+    return;
+  const int m0 = meas_offset[f], m = meas_offset[f + 1] - m0;
+  double pf[3] = {0.0, 0.0, 0.0};
+  const int ok = (m >= 2) ? triangulate_feature(m, meas_clone + m0, Rc, pc, uvn + 2 * (size_t)m0, o, pf) : 0;
+  status[f] = ok;
+  for (int i = 0; i < 3; i++)
+    p_FinG[3 * (size_t)f + i] = pf[i];
+}
+
+// the caller's options, or FeatureInitializerOptions' defaults (ov_core) when there are none
+static TriOptions tri_options(const ovp_triangulation_options *q) {
+  if (!q)
+    return {5, 1e-3, 1e10, 1e-6, 1e-6, 10.0, 0.10, 60.0, 40.0, 10000.0};
+  return {q->max_runs, q->init_lamda, q->max_lamda, q->min_dx, q->min_dcost, q->lam_mult, q->min_dist, q->max_dist, q->max_baseline, q->max_cond_number};
+}
+
+// counted copies between the host and slice `at` of the staging buffer d (nothing to copy: no call)
+static int stage_copy_in(Ctx *c, char *d, size_t at, const void *src, size_t bytes) {
+  if (bytes == 0)
+    return OVP_OK;
+  OVP_CUDA(cudaMemcpyAsync(d + at, src, bytes, cudaMemcpyHostToDevice, c->stream));
+  c->h2d_bytes += (int64_t)bytes;
+  return OVP_OK;
+}
+static int stage_copy_out(Ctx *c, void *dst, const char *d, size_t at, size_t bytes) {
+  if (bytes == 0)
+    return OVP_OK;
+  OVP_CUDA(cudaMemcpyAsync(dst, d + at, bytes, cudaMemcpyDeviceToHost, c->stream));
+  c->d2h_bytes += (int64_t)bytes;
+  return OVP_OK;
+}
+
+// camera pose table indexed by handle (R_GtoC: 9 doubles, p_CinG: 3) for the nh = c->vars.size() handles of the context
+struct PoseTable {
+  size_t R, p;
+  PoseTable(StageLayout &L, int nh) : R(L.take((size_t)nh * 72)), p(L.take((size_t)nh * 24)) {}
+};
+static void launch_cam_poses(Ctx *c, char *d, const PoseTable &t) { // launch errors surface at the stage launcher that reads the table
+  const int nh = (int)c->vars.size();
+  cam_pose_kernel<<<(nh + 127) / 128, 128, 0, c->stream>>>(nh, c->d_var_kind, c->d_var_id, c->d_val, c->h_calib, (double *)(d + t.R), (double *)(d + t.p));
+  c->launches++;
+}
+
+// F tracks (meas_offset: F + 1 entries) against the pose table t -> p_FinG (F x 3), status (F)
+static int launch_triangulate(Ctx *c, int F, const int *meas_offset, const int *meas_clone, const float *uvn, const TriOptions &o, char *d,
+                              const PoseTable &t, double *p_FinG, int *status) {
+  triangulate_kernel<<<(F + 63) / 64, 64, 0, c->stream>>>(F, meas_offset, meas_clone, uvn, (const double *)(d + t.R), (const double *)(d + t.p), o,
+                                                          p_FinG, status);
+  c->launches++;
+  OVP_CUDA(cudaGetLastError());
+  return OVP_OK;
+}
+
+// RANSAC's draws for a batch of planes (feat_offset: n_planes + 1 host entries): the PF_HYP permutations of every distinct point count once
+// (perms), the offset of plane p's in perm_off[p], and the largest count (it sizes plane_ransac_kernel's shared memory)
+struct RansacPlan {
+  std::vector<int> perm_off, perms;
+  int Fmax = 0;
+  RansacPlan(int n_planes, const int *feat_offset, int shuffle_kind) : perm_off(n_planes) {
+    std::map<int, int> at; // point count -> offset (ints) into perms
+    size_t n_ints = 0;
+    for (int p = 0; p < n_planes; p++) {
+      const int F = feat_offset[p + 1] - feat_offset[p];
+      Fmax = std::max(Fmax, F);
+      auto it = at.find(F);
+      if (it == at.end()) {
+        it = at.emplace(F, (int)n_ints).first;
+        n_ints += (size_t)PF_HYP * F;
+      }
+      perm_off[p] = it->second;
+    }
+    perms.resize(n_ints);
+    for (auto &kv : at)
+      pf_permutations_copy(kv.first, shuffle_kind, perms.data() + kv.second);
+  }
+};
+// RANSAC's outputs for up to n_planes planes of n_points points in all: hypotheses, selection scratch, status, abcd, inlier flags
+struct RansacOut {
+  size_t hyp, work, status, abcd, inlier;
+  RansacOut(StageLayout &L, int n_planes, int n_points)
+      : hyp(L.take((size_t)n_planes * PF_HYP * sizeof(PfHyp))), work(L.take((size_t)n_points * 32)), status(L.take((size_t)n_planes * 4)),
+        abcd(L.take((size_t)n_planes * 32)), inlier(L.take((size_t)n_points * 4)) {}
+};
+// the draws of every plane (perms / perm_off: RansacPlan's, on the device), then the winner of each
+static int launch_plane_ransac(Ctx *c, int n_planes, int Fmax, const int *feat_offset, const double *pts, const int *perms, const int *perm_off,
+                               double max_cond, int min_inliers, char *d, const RansacOut &o) {
+  const size_t smem = (size_t)Fmax * 24 + PF_WARPS * 20 * 8;
+  plane_ransac_kernel<<<dim3((PF_HYP + PF_WARPS - 1) / PF_WARPS, n_planes), 32 * PF_WARPS, smem, c->stream>>>(feat_offset, pts, perms, perm_off,
+                                                                                                              max_cond, (PfHyp *)(d + o.hyp));
+  plane_ransac_select_kernel<<<n_planes, 32, 0, c->stream>>>(feat_offset, pts, (const PfHyp *)(d + o.hyp), min_inliers, (double *)(d + o.work),
+                                                             (int *)(d + o.status), (double *)(d + o.abcd), (int *)(d + o.inlier));
+  c->launches += 2;
+  OVP_CUDA(cudaGetLastError());
+  return OVP_OK;
+}
+
+// the refinement's outputs for up to n_planes planes of n_points features in all
+struct RefineOut {
+  size_t scratch, p, cp, info, inlier, status;
+  RefineOut(StageLayout &L, int n_planes, int n_points)
+      : scratch(L.take((size_t)n_points * PO_FIELDS * 8)), p(L.take((size_t)n_points * 24)), cp(L.take((size_t)n_planes * 24)),
+        info(L.take((size_t)n_planes * 40)), inlier(L.take((size_t)n_points * 4)), status(L.take((size_t)n_planes * 4)) {}
+};
+// optimize_plane_kernel on n_planes planes, inputs on the device as ovp_optimize_plane takes them, camera poses from t.  The current camera
+// pose of the in-front-of-camera test (stateI, calib0: PlaneFitting.cpp:441-450) comes from the host mirror: sync_host_values first.
+static int launch_optimize_plane(Ctx *c, int n_planes, const int *feat_offset, const int *meas_offset, const int *meas_clone, const float *uvn,
+                                 const double *p0, const double *cp0, const int *fix_plane, double sigma_px_norm, double sigma_c, int max_iter,
+                                 char *d, const PoseTable &t, const RefineOut &o) {
+  PoArgs A;
+  const double *vi = c->h_val.data() + (size_t)c->h_imu * OVP_VAL_STRIDE, *vc = c->h_val.data() + (size_t)c->h_calib * OVP_VAL_STRIDE;
+  double Ri[9], RC[9];
+  quat_to_rot(vi, Ri);
+  quat_to_rot(vc, RC);
+  mat3_mul(RC, Ri, A.R_cur);
+  for (int i = 0; i < 3; i++)
+    A.p_cur[i] = vi[4 + i] - (A.R_cur[i] * vc[4] + A.R_cur[3 + i] * vc[5] + A.R_cur[6 + i] * vc[6]);
+  A.feat_offset = feat_offset;
+  A.meas_offset = meas_offset;
+  A.meas_clone = meas_clone;
+  A.fix_plane = fix_plane;
+  A.uvn = uvn;
+  A.p0 = p0;
+  A.cp0 = cp0;
+  A.Rc = (const double *)(d + t.R);
+  A.pc = (const double *)(d + t.p);
+  A.sigma_px_norm = sigma_px_norm;
+  A.sigma_c = sigma_c;
+  A.max_iter = max_iter;
+  A.scratch = (double *)(d + o.scratch);
+  A.p_out = (double *)(d + o.p);
+  A.cp_out = (double *)(d + o.cp);
+  A.info = (double *)(d + o.info);
+  A.inlier = (int *)(d + o.inlier);
+  A.status = (int *)(d + o.status);
+  optimize_plane_kernel<<<n_planes, PO_THREADS, 0, c->stream>>>(A);
+  c->launches++;
+  OVP_CUDA(cudaGetLastError());
+  return OVP_OK;
+}
+
 } // namespace ovp
 
 extern "C" {
+
+int ovp_triangulate_features(ovp_ctx *h, int F, const int *meas_offset, const int *meas_clone, const float *uv_norm,
+                             const ovp_triangulation_options *opt, double *p_FinG, int *status) {
+  using namespace ovp;
+  Ctx *c = ovp::enter(h);
+  if (F <= 0)
+    return OVP_OK;
+  if (!meas_offset || !meas_clone || !uv_norm || !p_FinG || !status)
+    return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: null argument");
+  const int M = meas_offset[F];
+  for (int k = 0; k < M; k++)
+    if (!is_clone(c, meas_clone[k], true))
+      return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: measurement %d: handle %d is not a clone in the state", k, meas_clone[k]);
+  if (c->var_table_dirty) {
+    int st = upload_var_table(c);
+    if (st)
+      return st;
+  }
+  // staging: [offsets | clones | uvn] in, [p_FinG | status] out, camera pose table
+  StageLayout L;
+  const size_t b_off = L.take((size_t)(F + 1) * 4), b_cl = L.take((size_t)M * 4), b_uv = L.take((size_t)M * 8), b_pf = L.take((size_t)F * 24),
+               b_st = L.take((size_t)F * 4);
+  const PoseTable pose(L, (int)c->vars.size());
+  int st = ensure_stage(c, L.top / 8 + 8);
+  if (st)
+    return st;
+  char *d = (char *)c->d_stage;
+  if ((st = stage_copy_in(c, d, b_off, meas_offset, (size_t)(F + 1) * 4)) || (st = stage_copy_in(c, d, b_cl, meas_clone, (size_t)M * 4)) ||
+      (st = stage_copy_in(c, d, b_uv, uv_norm, (size_t)M * 8)))
+    return st;
+  launch_cam_poses(c, d, pose);
+  if ((st = launch_triangulate(c, F, (const int *)(d + b_off), (const int *)(d + b_cl), (const float *)(d + b_uv), tri_options(opt), d, pose,
+                               (double *)(d + b_pf), (int *)(d + b_st))) ||
+      (st = stage_copy_out(c, p_FinG, d, b_pf, (size_t)F * 24)) || (st = stage_copy_out(c, status, d, b_st, (size_t)F * 4)))
+    return st;
+  OVP_CUDA(cudaStreamSynchronize(c->stream));
+  return OVP_OK;
+}
 
 int ovp_plane_shuffle(int n, int n_shuffles, int shuffle_kind, int *out) {
   if (n < 0 || n_shuffles < 0 || !out || (shuffle_kind != 0 && shuffle_kind != 1))
@@ -1034,21 +1237,10 @@ int ovp_plane_fitting(ovp_ctx *h, int n_planes, const int *feat_offset, const do
   if (feat_offset[0] != 0)
     return fail(c, OVP_ERR_BAD_ARGS, "plane_fitting: feat_offset must start at 0");
   const int Ftot = feat_offset[n_planes];
-  int Fmax = 0;
-  std::map<int, int> perm_off; // F -> offset (ints) into the permutation block of this call
-  std::vector<int> h_perm_off(n_planes);
-  size_t perm_ints = 0;
   for (int p = 0; p < n_planes; p++) {
     const int F = feat_offset[p + 1] - feat_offset[p];
     if (F < 0 || F > PF_MAX_POINTS)
       return fail(c, OVP_ERR_CAPACITY, "plane_fitting: plane %d has %d points (limit %d)", p, F, PF_MAX_POINTS);
-    Fmax = std::max(Fmax, F);
-    auto it = perm_off.find(F);
-    if (it == perm_off.end()) {
-      it = perm_off.emplace(F, (int)perm_ints).first;
-      perm_ints += (size_t)PF_HYP * F;
-    }
-    h_perm_off[p] = it->second;
   }
   if (Ftot == 0) {
     for (int p = 0; p < n_planes; p++) {
@@ -1058,36 +1250,28 @@ int ovp_plane_fitting(ovp_ctx *h, int n_planes, const int *feat_offset, const do
     }
     return OVP_OK;
   }
-  // staging (bytes): [feat_offset | perm_off | perms | pts] in, [hyp | work | status | abcd | inlier] out
-  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t b_fo = 0, b_po = al(b_fo + (size_t)(n_planes + 1) * 4), b_pm = al(b_po + (size_t)n_planes * 4), b_pt = al(b_pm + perm_ints * 4);
-  const size_t b_in_end = al(b_pt + (size_t)Ftot * 24);
-  const size_t b_hy = b_in_end, b_wk = al(b_hy + (size_t)n_planes * PF_HYP * sizeof(PfHyp)), b_st = al(b_wk + (size_t)Ftot * 32);
-  const size_t b_ab = al(b_st + (size_t)n_planes * 4), b_il = al(b_ab + (size_t)n_planes * 32), b_end = al(b_il + (size_t)Ftot * 4);
-  int st = ensure_stage(c, b_end / 8 + 8);
+  const RansacPlan plan(n_planes, feat_offset, opt->shuffle_kind);
+  // staging (bytes): [feat_offset | perm_off | perms | pts] in, RANSAC's outputs
+  StageLayout L;
+  const size_t b_fo = L.take((size_t)(n_planes + 1) * 4), b_po = L.take((size_t)n_planes * 4), b_pm = L.take(plan.perms.size() * 4),
+               b_pt = L.take((size_t)Ftot * 24), b_in_end = L.top;
+  const RansacOut out(L, n_planes, Ftot);
+  int st = ensure_stage(c, L.top / 8 + 8);
   if (st)
     return st;
   std::vector<char> hbuf(b_in_end);
   std::memcpy(hbuf.data() + b_fo, feat_offset, (size_t)(n_planes + 1) * 4);
-  std::memcpy(hbuf.data() + b_po, h_perm_off.data(), (size_t)n_planes * 4);
-  for (auto &kv : perm_off)
-    pf_permutations_copy(kv.first, opt->shuffle_kind, (int *)(hbuf.data() + b_pm + (size_t)kv.second * 4));
+  std::memcpy(hbuf.data() + b_po, plan.perm_off.data(), (size_t)n_planes * 4);
+  std::memcpy(hbuf.data() + b_pm, plan.perms.data(), plan.perms.size() * 4);
   std::memcpy(hbuf.data() + b_pt, p_FinG, (size_t)Ftot * 24);
   char *d = (char *)c->d_stage;
-  OVP_CUDA(cudaMemcpyAsync(d, hbuf.data(), b_in_end, cudaMemcpyHostToDevice, c->stream));
-  c->h2d_bytes += (int64_t)b_in_end;
-  const size_t smem = (size_t)Fmax * 24 + PF_WARPS * 20 * 8;
-  plane_ransac_kernel<<<dim3((PF_HYP + PF_WARPS - 1) / PF_WARPS, n_planes), 32 * PF_WARPS, smem, c->stream>>>(
-      (const int *)(d + b_fo), (const double *)(d + b_pt), (const int *)(d + b_pm), (const int *)(d + b_po), opt->max_cond_number, (PfHyp *)(d + b_hy));
-  plane_ransac_select_kernel<<<n_planes, 32, 0, c->stream>>>((const int *)(d + b_fo), (const double *)(d + b_pt), (const PfHyp *)(d + b_hy), opt->min_inlier_num,
-                                                             (double *)(d + b_wk), (int *)(d + b_st), (double *)(d + b_ab), (int *)(d + b_il));
-  c->launches += 2;
-  OVP_CUDA(cudaGetLastError());
-  OVP_CUDA(cudaMemcpyAsync(status, d + b_st, (size_t)n_planes * 4, cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(abcd, d + b_ab, (size_t)n_planes * 32, cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(inlier, d + b_il, (size_t)Ftot * 4, cudaMemcpyDeviceToHost, c->stream));
+  if ((st = stage_copy_in(c, d, 0, hbuf.data(), b_in_end)) ||
+      (st = launch_plane_ransac(c, n_planes, plan.Fmax, (const int *)(d + b_fo), (const double *)(d + b_pt), (const int *)(d + b_pm),
+                                (const int *)(d + b_po), opt->max_cond_number, opt->min_inlier_num, d, out)) ||
+      (st = stage_copy_out(c, status, d, out.status, (size_t)n_planes * 4)) || (st = stage_copy_out(c, abcd, d, out.abcd, (size_t)n_planes * 32)) ||
+      (st = stage_copy_out(c, inlier, d, out.inlier, (size_t)Ftot * 4)))
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream)); // hbuf is pageable: the H2D copy above has completed by now as well
-  c->d2h_bytes += (int64_t)n_planes * 36 + (int64_t)Ftot * 4;
   return OVP_OK;
 }
 
@@ -1114,11 +1298,9 @@ int ovp_optimize_plane(ovp_ctx *h, int n_planes, const int *feat_offset, const i
     return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: null measurement arrays");
   if (!(opt->sigma_px_norm > 0.0) || !(opt->sigma_c > 0.0))
     return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: sigma_px_norm / sigma_c must be positive");
-  for (int k = 0; k < M; k++) {
-    const int hh = meas_clone[k];
-    if (hh < 0 || hh >= (int)c->vars.size() || !c->vars[hh].alive || c->vars[hh].kind != OVP_KIND_POSE || c->vars[hh].id < 0 || hh == c->h_calib)
-      return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: measurement %d: handle %d is not a clone in the state", k, hh);
-  }
+  for (int k = 0; k < M; k++)
+    if (!is_clone(c, meas_clone[k], true))
+      return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: measurement %d: handle %d is not a clone in the state", k, meas_clone[k]);
   if (Ftot == 0) {
     for (int p = 0; p < n_planes; p++) {
       status[p] = 0;
@@ -1135,27 +1317,17 @@ int ovp_optimize_plane(ovp_ctx *h, int n_planes, const int *feat_offset, const i
     if (st)
       return st;
   }
-  int st = sync_host_values(c); // current IMU pose + extrinsics for the in-front-of-camera test (stateI, calib0: PlaneFitting.cpp:441-450)
+  int st = sync_host_values(c); // the current IMU pose and the extrinsics of the in-front-of-camera test
   if (st)
     return st;
-  PoArgs A;
-  {
-    const double *vi = c->h_val.data() + (size_t)c->h_imu * OVP_VAL_STRIDE, *vc = c->h_val.data() + (size_t)c->h_calib * OVP_VAL_STRIDE;
-    double Ri[9], RC[9];
-    quat_to_rot(vi, Ri);
-    quat_to_rot(vc, RC);
-    mat3_mul(RC, Ri, A.R_cur);
-    for (int i = 0; i < 3; i++)
-      A.p_cur[i] = vi[4 + i] - (A.R_cur[i] * vc[4] + A.R_cur[3 + i] * vc[5] + A.R_cur[6 + i] * vc[6]);
-  }
-  const int nh = (int)c->vars.size();
-  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t b_fo = 0, b_mo = al(b_fo + (size_t)(n_planes + 1) * 4), b_mc = al(b_mo + (size_t)(Ftot + 1) * 4), b_uv = al(b_mc + (size_t)M * 4);
-  const size_t b_fx = al(b_uv + (size_t)M * 8), b_p0 = al(b_fx + (size_t)n_planes * 4), b_c0 = al(b_p0 + (size_t)Ftot * 24), b_in_end = al(b_c0 + (size_t)n_planes * 24);
-  const size_t b_R = b_in_end, b_pc = al(b_R + (size_t)nh * 72), b_sc = al(b_pc + (size_t)nh * 24), b_po = al(b_sc + (size_t)Ftot * PO_FIELDS * 8);
-  const size_t b_co = al(b_po + (size_t)Ftot * 24), b_if = al(b_co + (size_t)n_planes * 24), b_il = al(b_if + (size_t)n_planes * 40);
-  const size_t b_st = al(b_il + (size_t)Ftot * 4), b_end = al(b_st + (size_t)n_planes * 4);
-  st = ensure_stage(c, b_end / 8 + 8);
+  // staging: [feat_offset | meas_offset | meas_clone | uvn | fix | p0 | cp0] in, camera pose table, the refinement's outputs
+  StageLayout L;
+  const size_t b_fo = L.take((size_t)(n_planes + 1) * 4), b_mo = L.take((size_t)(Ftot + 1) * 4), b_mc = L.take((size_t)M * 4),
+               b_uv = L.take((size_t)M * 8), b_fx = L.take((size_t)n_planes * 4), b_p0 = L.take((size_t)Ftot * 24),
+               b_c0 = L.take((size_t)n_planes * 24), b_in_end = L.top;
+  const PoseTable pose(L, (int)c->vars.size());
+  const RefineOut out(L, n_planes, Ftot);
+  st = ensure_stage(c, L.top / 8 + 8);
   if (st)
     return st;
   std::vector<char> hbuf(b_in_end);
@@ -1169,38 +1341,17 @@ int ovp_optimize_plane(ovp_ctx *h, int n_planes, const int *feat_offset, const i
   std::memcpy(hbuf.data() + b_p0, p_FinG, (size_t)Ftot * 24);
   std::memcpy(hbuf.data() + b_c0, cp_inG, (size_t)n_planes * 24);
   char *d = (char *)c->d_stage;
-  OVP_CUDA(cudaMemcpyAsync(d, hbuf.data(), b_in_end, cudaMemcpyHostToDevice, c->stream));
-  c->h2d_bytes += (int64_t)b_in_end;
-  cam_pose_kernel<<<(nh + 127) / 128, 128, 0, c->stream>>>(nh, c->d_var_kind, c->d_var_id, c->d_val, c->h_calib, (double *)(d + b_R), (double *)(d + b_pc));
-  A.feat_offset = (const int *)(d + b_fo);
-  A.meas_offset = (const int *)(d + b_mo);
-  A.meas_clone = (const int *)(d + b_mc);
-  A.fix_plane = (const int *)(d + b_fx);
-  A.uvn = (const float *)(d + b_uv);
-  A.p0 = (const double *)(d + b_p0);
-  A.cp0 = (const double *)(d + b_c0);
-  A.Rc = (const double *)(d + b_R);
-  A.pc = (const double *)(d + b_pc);
-  A.sigma_px_norm = opt->sigma_px_norm;
-  A.sigma_c = opt->sigma_c;
-  A.max_iter = opt->max_num_iterations > 0 ? opt->max_num_iterations : 12; // PlaneFitting.cpp:396
-  A.scratch = (double *)(d + b_sc);
-  A.p_out = (double *)(d + b_po);
-  A.cp_out = (double *)(d + b_co);
-  A.info = (double *)(d + b_if);
-  A.inlier = (int *)(d + b_il);
-  A.status = (int *)(d + b_st);
-  optimize_plane_kernel<<<n_planes, PO_THREADS, 0, c->stream>>>(A);
-  c->launches += 2;
-  OVP_CUDA(cudaGetLastError());
-  OVP_CUDA(cudaMemcpyAsync(p_FinG_out, d + b_po, (size_t)Ftot * 24, cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(cp_out, d + b_co, (size_t)n_planes * 24, cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(inlier, d + b_il, (size_t)Ftot * 4, cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(status, d + b_st, (size_t)n_planes * 4, cudaMemcpyDeviceToHost, c->stream));
-  if (info)
-    OVP_CUDA(cudaMemcpyAsync(info, d + b_if, (size_t)n_planes * 40, cudaMemcpyDeviceToHost, c->stream));
+  if ((st = stage_copy_in(c, d, 0, hbuf.data(), b_in_end)))
+    return st;
+  launch_cam_poses(c, d, pose);
+  if ((st = launch_optimize_plane(c, n_planes, (const int *)(d + b_fo), (const int *)(d + b_mo), (const int *)(d + b_mc), (const float *)(d + b_uv),
+                                  (const double *)(d + b_p0), (const double *)(d + b_c0), (const int *)(d + b_fx), opt->sigma_px_norm, opt->sigma_c,
+                                  opt->max_num_iterations > 0 ? opt->max_num_iterations : 12, d, pose, out)) || // PlaneFitting.cpp:396
+      (st = stage_copy_out(c, p_FinG_out, d, out.p, (size_t)Ftot * 24)) || (st = stage_copy_out(c, cp_out, d, out.cp, (size_t)n_planes * 24)) ||
+      (st = stage_copy_out(c, inlier, d, out.inlier, (size_t)Ftot * 4)) || (st = stage_copy_out(c, status, d, out.status, (size_t)n_planes * 4)) ||
+      (info && (st = stage_copy_out(c, info, d, out.info, (size_t)n_planes * 40))))
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
-  c->d2h_bytes += (int64_t)Ftot * 28 + (int64_t)n_planes * (28 + (info ? 40 : 0));
   return OVP_OK;
 }
 

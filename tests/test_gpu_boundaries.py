@@ -250,6 +250,14 @@ def test_slam_refuses_tracks_beyond_the_limit(m, chi2_table):
     assert err.value.status == OVP_ERR_CAPACITY
     assert "%d measurements" % m in str(err.value) and "longest supported track is %d" % MAX_TRACK_SLAM in str(err.value)
     assert_state_unchanged(ctx, handles, snap)
+    calib_clone = tail_batch(ug, MAX_TRACK_SLAM)  # within the limit, but the camera extrinsics are a pose, not a clone
+    calib_clone["meas_clone"][0] = ctx.handle_calib()
+    l0 = ctx.launch_count()
+    with pytest.raises(api.OvpError) as err:
+        ctx.slam_update(calib_clone, 1.0, 1.0)
+    assert err.value.status == 1 and "not a clone" in str(err.value)
+    assert ctx.launch_count() == l0
+    assert_state_unchanged(ctx, handles, snap)
     _, e = _slam_update_and_compare(ctx, orc, tail_batch(ug, MAX_TRACK_SLAM), tail_batch(uo, MAX_TRACK_SLAM), g, o, keep)
     print("follow-up slam update at m=%d: cov rel err %.2e" % (MAX_TRACK_SLAM, e))
     ctx.close()

@@ -357,6 +357,17 @@ def test_error_codes(chi2_table):
     with pytest.raises(api.OvpError) as e:
         ctx.augment_clone(S.clones[0][0], np.zeros(3))
     assert e.value.status == 10  # OVP_ERR_TIME
+    # the camera extrinsics are a pose, not a clone: every entry point that takes clone handles refuses them before a copy or launch
+    cal, P0, l0 = ctx.handle_calib(), ctx.cov(), ctx.launch_count()
+    uv, p = np.zeros((2, 2)), np.array([0.0, 0.0, 2.0])
+    for call in (lambda: ctx.feature_jacobian_full([chg[0], cal], uv, p, p, 0, None, None, 1.0, 0.01),
+                 lambda: ctx.msckf_shard_columns([chg[0], cal]),
+                 lambda: ctx.triangulate_features([0, 2], [chg[0], cal], uv),
+                 lambda: ctx.optimize_plane([0, 1], [0, 2], [chg[0], cal], uv, p[None], np.array([[0.0, 0.0, 1.0]]), [0], 1.0 / 458.0, 0.01)):
+        with pytest.raises(api.OvpError) as e:
+            call()
+        assert e.value.status == 1 and "not a clone" in str(e.value)
+    assert ctx.launch_count() == l0 and np.array_equal(ctx.cov(), P0)
     # a negative-diagonal covariance is reported (reference: std::exit)
     P = ctx.cov()
     P[3, 3] = -1.0

@@ -159,6 +159,8 @@ def test_refusals_launch_nothing_and_leave_the_state_as_it_was(chi2_table):
         return v
     bad_clone = variant()
     bad_clone["meas_clone"][a0] = ctx.handle_imu()
+    calib_clone = variant()  # the camera extrinsics are a pose, not a clone
+    calib_clone["meas_clone"][a0] = ctx.handle_calib()
     dup = variant()
     dup["featid"][cand[1]] = dup["featid"][f0]
     # one candidate with 38 measurements (one above the plane-system limit)
@@ -172,7 +174,7 @@ def test_refusals_launch_nothing_and_leave_the_state_as_it_was(chi2_table):
                    meas_clone=np.concatenate([t["meas_clone"][:sl.start], mc_f, t["meas_clone"][sl.stop:]]).astype(np.int32),
                    uv=np.concatenate([t["uv"][:sl.start], uv_f, t["uv"][sl.stop:]]).astype(np.float32),
                    uv_norm=np.concatenate([t["uv_norm"][:sl.start], uvn_f, t["uv_norm"][sl.stop:]]).astype(np.float32))
-    cases = [(bad_clone, {}, api.OvpError, 1), (dup, {}, api.OvpError, 1), (long, {}, api.OvpError, 7), (t, dict(max_msckf_plane=5000), api.OvpError, 7),
+    cases = [(bad_clone, {}, api.OvpError, 1), (calib_clone, {}, api.OvpError, 1), (dup, {}, api.OvpError, 1), (long, {}, api.OvpError, 7), (t, dict(max_msckf_plane=5000), api.OvpError, 7),
              (t, dict(shuffle_kind=3), api.OvpError, 1)]
     P0, v0, o0 = _state(ctx)
     l0 = ctx.launch_count()

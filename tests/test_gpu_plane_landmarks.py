@@ -250,6 +250,13 @@ def test_refusals_leave_the_state_untouched(chi2_table):
         with pytest.raises(api.OvpError) as e:
             ctx.msckf_update_landmarks(bg, f, p)
         assert "landmark" in str(e.value)
+    calib_clone = dict(bg, meas_clone=bg["meas_clone"].copy())  # the camera extrinsics are a pose, not a clone
+    calib_clone["meas_clone"][0] = ctx.handle_calib()
+    l0 = ctx.launch_count()
+    with pytest.raises(api.OvpError) as e:
+        ctx.msckf_update(calib_clone)
+    assert e.value.status == 1 and "not a clone" in str(e.value)
+    assert ctx.launch_count() == l0
     ctx.slam_set_representation(int(fids[0]), 1, -1)  # not GLOBAL_3D
     with pytest.raises(api.OvpError) as e:
         ctx.msckf_update_landmarks(bg, fids, pids)
