@@ -156,8 +156,8 @@ int ovp_plane_measurement_compress_inplace(ovp_ctx *ctx, double *H_x, int cols, 
 
 /* ---- UpdaterMSCKF::update from "features triangulated, plane CPs known" on (UpdaterMSCKF.cpp:407-828) --------------- */
 /* Track length: every feature of a batch has 2..39 measurements, or 2..37 when the batch runs a plane update (an in-state plane,
- * a plane not in the state with >= 4 features, or ovp_plane_init).  Tracks of up to 32 run on one warp per feature; one longer
- * track puts the whole batch on one CTA per feature, whose per-feature system must fit the CTA's shared memory.  A longer track
+ * a plane not in the state with >= 4 features, or ovp_plane_init).  Tracks of up to 32 run on the block-sparse feature kernel; one
+ * longer track puts the whole batch on the dense stacked one, whose per-feature system must fit the CTA's shared memory.  A longer track
  * is refused with OVP_ERR_CAPACITY before anything is launched, and the message names the limit.  Every other capacity check
  * of the update (rows, columns, factorisation width) also runs before the first launch, so a refused batch leaves the state as
  * it was. */

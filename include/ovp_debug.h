@@ -42,7 +42,7 @@ int ovp_debug_gemm(ovp_ctx *ctx, int M, int N, int K, const double *A, int a_row
  * [c kc, min(K, (c + 1) kc)); one chunk is the unsplit k walk. */
 int ovp_debug_gemm_split(ovp_ctx *ctx, int M, int N, int K, int tri, int ktri, int tile, int *info);
 /* on != 0: every later ovp_msckf_update of this context builds its point and plane systems with the one-block-per-feature kernel and
- * the dense stacked Gram matrix, also when all its tracks fit the warp-per-feature path (at most 32 measurements) */
+ * the dense stacked Gram matrix, also when all its tracks fit the block-sparse path (at most 32 measurements) */
 int ovp_debug_force_dense_features(ovp_ctx *ctx, int on);
 /* on != 0: every later compressed update of this context forms M = P[:, cols] L and S = L^T M[cols, :] + I with two GEMM launches after
  * the factorisation of its Gram matrix, instead of inside that factorisation launch */
@@ -56,7 +56,7 @@ int ovp_debug_chol_products(ovp_ctx *ctx, const double *G, int nc, int npiv, dou
 /* prepare a feature batch as ovp_msckf_update does and run the first non-empty plan of its launch order (planes in ascending id, then the
  * point update) up to its Gram matrix G = [H_o r_o]^T [H_o r_o] of the nullspace-projected system; the state is left as it was.  G_out
  * (gcap * gcap doubles) receives all of G, nc1 x nc1 column-major: the ncx x columns (calibration, then 6 per clone), for a plane its
- * 3 H_cp columns, the residual last.  info[8] = {nc1, ncal, ncx, point plan, nsel, warp-per-feature path, plane slot, plane in the
+ * 3 H_cp columns, the residual last.  info[8] = {nc1, ncal, ncx, point plan, nsel, block-sparse path, plane slot, plane in the
  * state}.  cols_out (gcap): state index of every x column; sel_out (F): the nsel features of the plan; feat_status / feat_chi2 (F): the
  * per-feature status words after the plan's feature kernel (point plan: 1 accepted, 0 rejected by the gate).  raw_out (NULL, or 72
  * doubles per measurement of the batch): the raw whitened rows the feature kernel built, per measurement 3 rows of 24 doubles: the two

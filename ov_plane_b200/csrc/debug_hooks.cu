@@ -277,7 +277,7 @@ extern "C" int ovp_debug_chol_products(ovp_ctx *h, const double *G, int nc, int 
 // launch order (a plane plan first if the batch has planes, otherwise the point plan) up to its Gram matrix G = D - Y^T Y; nothing after
 // it runs, so the state is left as it was.  Eager launches.  G_out (gcap x gcap, column-major, leading dimension nc1) receives all of G.
 // info: [0] nc1, [1] ncal, [2] ncx (x columns; H_cp, when present, sits at ncx .. ncx + 2 and the residual at nc1 - 1), [3] point plan,
-// [4] selected features nsel, [5] warp-per-feature path, [6] plane slot, [7] plane in the state.  cols_out (gcap): compact column -> state
+// [4] selected features nsel, [5] CTA-per-feature path, [6] plane slot, [7] plane in the state.  cols_out (gcap): compact column -> state
 // index of the x columns; sel_out (F): the plan's features; feat_status / feat_chi2 (F): the per-feature status words after the plan's
 // feature kernel.  raw_out (optional, 3 * OVP_RAW_ROW doubles per measurement, OVP_RAW_ROW in features.cu): the raw whitened rows the
 // feature kernel built.  A plan that goes straight into the update (no compression) has no Gram matrix: OVP_ERR_BAD_ARGS.  Not part of

@@ -108,7 +108,7 @@ struct Ctx {
   int nccl_rank = 0, nccl_nranks = 1;
   double *d_gather = nullptr;  // nranks packed lower triangles
   size_t d_gather_elems = 0;
-  double *d_mw = nullptr;      // warp-per-feature path: measurement blocks, per-feature dense blocks, D part (msckf_warp.inc)
+  double *d_mw = nullptr;      // CTA-per-feature path: measurement blocks, per-feature dense blocks, D part (msckf_warp.inc)
   size_t d_mw_elems = 0;
   // feature batch staging
   void *d_batch = nullptr;
