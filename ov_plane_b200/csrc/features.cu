@@ -391,7 +391,8 @@ __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
 // Operand tiles are 64 columns of Hs x 16 rows (k), k contiguous in global memory AND in shared memory ([col][k], stride 20
 // doubles: 16-byte vector copies without bank conflicts, DMMA fragment reads (8 cols x 4 k) on 16 distinct 8-byte banks because
 // 20 mod 16 == 4); the next k-step is prefetched into registers while the current one is in the tensor pipe; a diagonal tile
-// loads its operand once.
+// loads its operand once.  The shape is m8n8k4, which runs at half the per-SM tensor rate of the m16n8 shapes on an H100 (gemm.cuh,
+// tools/lab/dmma_lab.cu); moving this kernel to m16n8k16 is open.
 #define GRAM_KS 20
 __global__ void __launch_bounds__(128) gram_kernel(const double *Hs, int ld, int rows, int nc, int kchunk, double *part, int ldp) {
   const int tm = blockIdx.y, tn = blockIdx.x;

@@ -2,8 +2,10 @@
 // M = P[:,ids] H^T, S = H M[ids,:] + R, the Cholesky trailing updates, the triangular-inverse merges, Y = M L^-T and
 // P -= Y Y^T (StateHelper.cpp:142-171 restructured, see DESIGN.md).  wgmma has no f64 kind, and the path needs fp64
 // (DESIGN.md "precision"), so the fp64 tensor-core work goes through warp-level mma.sync.  This kernel uses the m8n8k4 shape; sm_90
-// also has the f64 shapes m16n8k4 / m16n8k8 / m16n8k16, which have not been tried here (whether they beat m8n8k4 on an H100 is not
-// measured).
+// also has the f64 shapes m16n8k4 / m16n8k8 / m16n8k16, each a single DMMA instruction.  Measured on an H100 80GB HBM3 at a 700 W
+// power limit (tools/lab/dmma_lab.cu, one SM): m8n8k4 reaches 127 FP64 flops / cycle with 8 warps, every m16n8 shape 252-255, i.e.
+// m8n8k4 runs at HALF the tensor rate; dependent-chain latency 30 / 34 / 50 / 82 cycles for m8n8k4 / k4 / k8 / k16 (7.5 / 8.5 / 6.3 /
+// 5.1 cycles per unit of k).  The fused Cholesky (cholfused.cu) runs on m16n8k16; moving this kernel is open.
 //
 // Operands are strided views (element (i,k) = p[i*si + K(k)*sk], optional gather K(k) = kidx[k] along the contraction
 // dimension) so that transposes and the P[:, ids] / M[ids, :] gathers of EKFUpdate need no copies and no divergent code.  A CTA
@@ -33,6 +35,13 @@ __device__ __forceinline__ void dmma_m8n8k4(double &d0, double &d1, double a, do
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
                : "+d"(d0), "+d"(d1)
                : "d"(a), "d"(b));
+}
+// c += A B, A 16 x 16, B 16 x 8 (one DMMA.16x8x16).  With g = lane / 4, t = lane % 4:
+//   a[i] = A(g + 8 (i & 1), t + 4 (i >> 1)),   b[i] = B(t + 4 i, g),   c[i] = C(g + 8 (i >> 1), 2 t + (i & 1))
+__device__ __forceinline__ void dmma_m16n8k16(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
 }
 
 // Host-side logical matrix view: element (i,j) = p[row(i) + col(j)*ld] (after optional transpose), optional gather indices.
