@@ -426,7 +426,8 @@ int ovp_set_use_graphs(ovp_ctx *ctx, int on);
  * column's original diagonal entry) marks a rank-deficient (gauge) direction and is dropped.  Default 1e-11; the posterior is
  * invariant over 1e-9 .. 1e-13 on every scenario in tests/ (tests/test_gpu_numerics.py). */
 int ovp_set_rank_tolerance(ovp_ctx *ctx, double tol);
-/* bytes this ctx copied host->device / device->host since creation */
+/* bytes this ctx copied host->device / device->host since creation: every host<->device copy the library issues for the ctx (operands,
+ * results, column indices, variable tables and values, status words) is counted */
 int ovp_transfer_bytes(ovp_ctx *ctx, int64_t *h2d, int64_t *d2h);
 /* measured FP64 tensor-core (DMMA) throughput of this device with the library's own GEMM kernel: returns TFLOP/s */
 int ovp_selftest_dgemm_tflops(ovp_ctx *ctx, int n, int iters, double *tflops);

@@ -140,30 +140,28 @@ int ovp_feature_jacobian_full_rep(ovp_ctx *h, int m, const int *clone_handles, c
     if (clone_handles[i] == anchor_clone_handle)
       anchor_k = i;
   const int extra = (rel && anchor_k < 0) ? 6 : 0;
-  int rows, hfc, hxc;
-  st = stage_feature_jacobian(c, m, clone_handles, uv, pG, pGf, false, -1, nullptr, nullptr, sigma_px, 1.0, &rows, &hfc, &hxc, extra);
+  FeatureJacobianStage j;
+  st = stage_feature_jacobian(c, m, clone_handles, uv, pG, pGf, false, -1, nullptr, nullptr, sigma_px, 1.0, &j, extra);
   if (st)
     return st;
   const int ncal_pose = c->opt.do_calib_camera_pose ? 6 : 0, ncal = ncal_pose + (c->opt.do_calib_camera_intrinsics ? 8 : 0);
-  a.Hf = c->d_stage;
-  a.Hx = c->d_stage + (size_t)rows * hfc;
-  a.rows = rows;
+  a.Hf = j.W(c);
+  a.Hx = j.Hx(c);
+  a.rows = j.rows;
   a.k = k;
   a.anchor_col = rel ? (anchor_k >= 0 ? ncal + 6 * anchor_k : ncal + 6 * m) : -1;
   a.calib_col = (rel && ncal_pose) ? 0 : -1;
   if (!rel)
     for (int i = 0; i < 18; i++)
       a.Ha[i] = a.Hc[i] = 0.0;
-  representation_chain_kernel<<<(rows + 63) / 64, 64, 0, c->stream>>>(a);
+  representation_chain_kernel<<<(j.rows + 63) / 64, 64, 0, c->stream>>>(a);
   c->launches++;
   OVP_CUDA(cudaGetLastError());
-  OVP_CUDA(cudaMemcpyAsync(H_f, a.Hf, (size_t)rows * k * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(H_x, a.Hx, (size_t)rows * hxc * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(res, c->d_stage + (size_t)rows * (hfc + hxc), (size_t)rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaStreamSynchronize(c->stream));
+  if ((st = read_feature_jacobian(c, j, k, H_f, H_x, res)))
+    return st;
   *hf_cols = k;
-  *hx_cols = hxc;
-  *rows_out = rows;
+  *hx_cols = j.hxc;
+  *rows_out = j.rows;
   int no = 0;
   if (c->opt.do_calib_camera_pose)
     x_order[no++] = c->h_calib;

@@ -187,23 +187,6 @@ __global__ void dmma_selftest_fill(double *p, size_t n, double scale) {
     p[i] = scale * (double)((i * 2654435761u) % 1024) / 1024.0;
 }
 
-// host <-> device staging buffer for small dense transfers: grows on demand.  Only the staging buffer itself is replaced
-// (after the stream has drained: kernels in flight may still read it); snapshots, profiling events and the prepared batch
-// belong to other owners and are released in ovp_destroy.
-static int ensure_stage(Ctx *c, size_t elems) {
-  if (elems <= c->d_stage_elems)
-    return OVP_OK;
-  OVP_CUDA(cudaStreamSynchronize(c->stream));
-  if (c->d_stage)
-    cudaFree(c->d_stage);
-  c->d_stage = nullptr;
-  c->d_stage_elems = 0;
-  size_t n = std::max<size_t>(elems * 2, 1 << 16);
-  OVP_CUDA(cudaMalloc(&c->d_stage, n * sizeof(double)));
-  c->d_stage_elems = n;
-  return OVP_OK;
-}
-
 static int valid_handle(Ctx *c, int h) { return h >= 0 && h < (int)c->vars.size() && c->vars[h].alive; }
 
 // device array of state column indices for a list of handles (into c->dcols + slot*Rcap)
@@ -221,7 +204,9 @@ static int upload_cols(Ctx *c, const int *handles, int k, int slot, int *n_out, 
   if ((int)cols.size() > c->Rcap)
     return fail(c, OVP_ERR_CAPACITY, "%d columns exceed capacity %d", (int)cols.size(), c->Rcap);
   if (!cols.empty()) {
-    OVP_CUDA(cudaMemcpyAsync(c->dcols + (size_t)slot * c->Rcap, cols.data(), cols.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    int st = stage_copy_in(c, c->dcols + (size_t)slot * c->Rcap, cols.data(), cols.size() * sizeof(int));
+    if (st)
+      return st;
     OVP_CUDA(cudaStreamSynchronize(c->stream));
   }
   *n_out = (int)cols.size();
@@ -312,8 +297,8 @@ int ovp_create(const ovp_state_options *opt, int device, int max_state, int max_
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || device >= ndev)
     return OVP_ERR_CUDA; // no CPU fallback: the path needs a CUDA device
   ovp_ctx *h = new ovp_ctx();
+  h->c.device = device; // before enter: it makes this device current, and no other device gets a context
   Ctx *c = ovp::enter(h);
-  c->device = device;
   c->opt = *opt;
   *out = h;
   OVP_CUDA(cudaSetDevice(device));
@@ -448,16 +433,16 @@ int ovp_create(const ovp_state_options *opt, int device, int max_state, int max_
       P0[(size_t)(b + 4 + i) * cur + b + 4 + i] = std::pow(0.005, 2);
     }
   }
-  OVP_CUDA(cudaMemcpy2D(c->dP, (size_t)c->ldP * sizeof(double), P0.data(), (size_t)cur * sizeof(double), (size_t)cur * sizeof(double), cur,
-                        cudaMemcpyHostToDevice));
-  return upload_var_table(c);
+  st = stage_copy2d_in(c, c->dP, (size_t)c->ldP * sizeof(double), P0.data(), (size_t)cur * sizeof(double), (size_t)cur * sizeof(double), cur);
+  if (st)
+    return st;
+  return upload_var_table(c); // synchronises the stream
 }
 
 void ovp_destroy(ovp_ctx *h) {
   if (!h)
     return;
   Ctx *c = ovp::enter(h);
-  cudaSetDevice(c->device);
   if (c->stream)
     cudaStreamSynchronize(c->stream);
   cudaFree(c->dP);
@@ -519,7 +504,6 @@ int ovp_set_chi2_table(ovp_ctx *h, const double *q, int n) {
   Ctx *c = ovp::enter(h);
   if (!q || n < 2)
     return fail(c, OVP_ERR_BAD_ARGS, "chi2 table needs >= 2 entries");
-  OVP_CUDA(cudaSetDevice(c->device));
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   // a prepared batch (and its captured graph) holds the old table pointer and host-side thresholds by value: drop it
   free_prepared(c);
@@ -528,7 +512,9 @@ int ovp_set_chi2_table(ovp_ctx *h, const double *q, int n) {
     cudaFree(c->d_chi2_table);
   c->d_chi2_table = nullptr;
   OVP_CUDA(cudaMalloc(&c->d_chi2_table, n * sizeof(double)));
-  OVP_CUDA(cudaMemcpy(c->d_chi2_table, q, n * sizeof(double), cudaMemcpyHostToDevice));
+  int st = stage_copy_in(c, c->d_chi2_table, q, n * sizeof(double));
+  if (st)
+    return st;
   c->chi2_table_n = n;
   return OVP_OK;
 }
@@ -538,8 +524,9 @@ int ovp_cov_download(ovp_ctx *h, double *out, int ld) {
   Ctx *c = ovp::enter(h);
   if (ld < c->N)
     return fail(c, OVP_ERR_BAD_ARGS, "ld < rows");
-  OVP_CUDA(cudaMemcpy2DAsync(out, (size_t)ld * sizeof(double), c->dP, (size_t)c->ldP * sizeof(double), (size_t)c->N * sizeof(double), c->N,
-                             cudaMemcpyDeviceToHost, c->stream));
+  int st = stage_copy2d_out(c, out, (size_t)ld * sizeof(double), c->dP, (size_t)c->ldP * sizeof(double), (size_t)c->N * sizeof(double), c->N);
+  if (st)
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   return OVP_OK;
 }
@@ -547,8 +534,9 @@ int ovp_cov_upload(ovp_ctx *h, const double *in, int n, int ld) {
   Ctx *c = ovp::enter(h);
   if (n != c->N || ld < n)
     return fail(c, OVP_ERR_BAD_ARGS, "cov_upload: n=%d but the state has %d rows", n, c->N);
-  OVP_CUDA(cudaMemcpy2DAsync(c->dP, (size_t)c->ldP * sizeof(double), in, (size_t)ld * sizeof(double), (size_t)n * sizeof(double), n,
-                             cudaMemcpyHostToDevice, c->stream));
+  int st = stage_copy2d_in(c, c->dP, (size_t)c->ldP * sizeof(double), in, (size_t)ld * sizeof(double), (size_t)n * sizeof(double), n);
+  if (st)
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   return OVP_OK;
 }
@@ -677,12 +665,15 @@ int ovp_get_marginal_covariance(ovp_ctx *h, const int *handles, int k, double *o
     return st;
   if (n == 0)
     return OVP_OK;
-  st = ensure_stage(c, (size_t)n * n);
-  if (st)
+  StageLayout L;
+  const size_t b_blk = L.take((size_t)n * n * sizeof(double));
+  if ((st = ensure_stage(c, L)))
     return st;
-  gather_block_kernel<<<(n * n + 255) / 256, 256, 0, c->stream>>>(c->dP, c->ldP, c->dcols, n, c->d_stage);
+  double *blk = (double *)(c->d_stage + b_blk);
+  gather_block_kernel<<<(n * n + 255) / 256, 256, 0, c->stream>>>(c->dP, c->ldP, c->dcols, n, blk);
   c->launches++;
-  OVP_CUDA(cudaMemcpyAsync(out, c->d_stage, (size_t)n * n * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  if ((st = stage_copy_out(c, out, blk, (size_t)n * n * sizeof(double))))
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   return OVP_OK;
 }
@@ -694,11 +685,14 @@ int ovp_set_initial_covariance(ovp_ctx *h, const double *cov, int n_in, const in
     return st;
   if (n != n_in)
     return fail(c, OVP_ERR_BAD_ARGS, "set_initial_covariance: %d != sum of sizes %d", n_in, n);
-  st = ensure_stage(c, (size_t)n * n);
-  if (st)
+  StageLayout L;
+  const size_t b_blk = L.take((size_t)n * n * sizeof(double));
+  if ((st = ensure_stage(c, L)))
     return st;
-  OVP_CUDA(cudaMemcpyAsync(c->d_stage, cov, (size_t)n * n * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  scatter_block_kernel<<<(n * n + 255) / 256, 256, 0, c->stream>>>(c->dP, c->ldP, c->dcols, n, c->d_stage);
+  double *blk = (double *)(c->d_stage + b_blk);
+  if ((st = stage_copy_in(c, blk, cov, (size_t)n * n * sizeof(double))))
+    return st;
+  scatter_block_kernel<<<(n * n + 255) / 256, 256, 0, c->stream>>>(c->dP, c->ldP, c->dcols, n, blk);
   c->launches++;
   sym_from_upper_kernel<<<c->num_sms * 4, 256, 0, c->stream>>>(c->dP, c->ldP, c->N);
   c->launches++;
@@ -729,12 +723,14 @@ int ovp_ekf_propagation(ovp_ctx *h, const int *new_h, int kn, const int *old_h, 
   if (size_new > c->Rcap || size_old > c->Rcap)
     return fail(c, OVP_ERR_CAPACITY, "EKFPropagation: block too large");
   const int N = c->N, start = c->vars[new_h[0]].id;
-  st = ensure_stage(c, (size_t)phi_rows * phi_cols + (size_t)phi_rows * phi_rows);
-  if (st)
+  StageLayout L;
+  const size_t phi_bytes = (size_t)phi_rows * phi_cols * sizeof(double), q_bytes = (size_t)phi_rows * phi_rows * sizeof(double);
+  const size_t b_phi = L.take(phi_bytes), b_q = L.take(q_bytes);
+  if ((st = ensure_stage(c, L)))
     return st;
-  double *dPhi = c->d_stage, *dQ = c->d_stage + (size_t)phi_rows * phi_cols;
-  OVP_CUDA(cudaMemcpyAsync(dPhi, Phi, (size_t)phi_rows * phi_cols * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(dQ, Q, (size_t)phi_rows * phi_rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  double *dPhi = (double *)(c->d_stage + b_phi), *dQ = (double *)(c->d_stage + b_q);
+  if ((st = stage_copy_in(c, dPhi, Phi, phi_bytes)) || (st = stage_copy_in(c, dQ, Q, q_bytes)))
+    return st;
   sym_from_upper_kernel<<<8, 256, 0, c->stream>>>(dQ, phi_rows, phi_rows); // Q.selfadjointView<Upper>() (:93)
   c->launches++;
   // Cov_PhiT = P[:, old] Phi^T   (N x kn)

@@ -90,12 +90,12 @@ static int init_invertible_core(Ctx *c, int kind, int s, const double *value, co
     launch_gemm1(c, p);
   }
   // bring the s x s pieces to the host: H_finit (upper-triangular top of H_L), Mm, resinit
-  double hHL[9], hMm[9], hres[3], hW[3 * 3 + 3];
-  OVP_CUDA(cudaMemcpy2DAsync(hHL, s * sizeof(double), W, (size_t)ldW * sizeof(double), s * sizeof(double), s, cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(hMm, dMm, s * s * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(hres, W + (size_t)(s + n) * ldW, s * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  double hHL[9], hMm[9], hres[3];
+  int st;
+  if ((st = stage_copy2d_out(c, hHL, s * sizeof(double), W, (size_t)ldW * sizeof(double), s * sizeof(double), s)) ||
+      (st = stage_copy_out(c, hMm, dMm, s * s * sizeof(double))) || (st = stage_copy_out(c, hres, W + (size_t)(s + n) * ldW, s * sizeof(double))))
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
-  (void)hW;
   if (hl_is_upper) // called from initialize(): the reflectors annihilated the below-diagonal entries (the storage holds reflector data there);
     for (int j = 0; j < s; j++) // a direct ovp_initialize_invertible call hands over a general square H_L (StateHelper.cpp:564)
       for (int i = j + 1; i < s; i++)
@@ -133,7 +133,8 @@ static int init_invertible_core(Ctx *c, int kind, int s, const double *value, co
   double pack[18];
   std::memcpy(pack, Hinv, sizeof(double) * 9);
   std::memcpy(pack + 9, PLL, sizeof(double) * 9);
-  OVP_CUDA(cudaMemcpyAsync(dsm, pack, sizeof(pack), cudaMemcpyHostToDevice, c->stream));
+  if ((st = stage_copy_in(c, dsm, pack, sizeof(pack))))
+    return st;
   init_grow_kernel<<<((N + s) * s + 255) / 256, 256, 0, c->stream>>>(c->dP, c->ldP, N, s, c->dM, c->Nmax, dsm, dsm + 9);
   c->launches++;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
@@ -147,7 +148,7 @@ static int init_invertible_core(Ctx *c, int kind, int s, const double *value, co
     nv[i] = value[i] + dxn[i]; // new_variable->update(H_Linv * res), :577
     nf[i] = fej[i];
   }
-  int st = state_append_variable(c, v, nv, nf, new_handle);
+  st = state_append_variable(c, v, nv, nf, new_handle);
   if (st)
     return st;
   register_new(c, *new_handle, kind, tag);
@@ -156,14 +157,16 @@ static int init_invertible_core(Ctx *c, int kind, int s, const double *value, co
 
 // shared front half of initialize / initialize_invertible: stage W = [H_L | H_R | res] on the device
 static int stage_init_system(Ctx *c, const double *H_R, const double *H_L, const double *res, int rows, int n, int s, double **W) {
-  size_t e = (size_t)rows * (s + n + 1);
-  int st = ensure_stage(c, e + 64);
+  const size_t col = (size_t)rows * sizeof(double);
+  StageLayout L;
+  const size_t b_W = L.take(col * (s + n + 1));
+  int st = ensure_stage(c, L);
   if (st)
     return st;
-  *W = c->d_stage;
-  OVP_CUDA(cudaMemcpyAsync(*W, H_L, (size_t)rows * s * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(*W + (size_t)rows * s, H_R, (size_t)rows * n * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(*W + (size_t)rows * (s + n), res, (size_t)rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  *W = (double *)(c->d_stage + b_W);
+  if ((st = stage_copy_in(c, *W, H_L, col * s)) || (st = stage_copy_in(c, *W + (size_t)rows * s, H_R, col * n)) ||
+      (st = stage_copy_in(c, *W + (size_t)rows * (s + n), res, col)))
+    return st;
   return OVP_OK;
 }
 
@@ -181,21 +184,21 @@ int ovp_ekf_update(ovp_ctx *h, const int *handles, int k, const double *H, int r
     return fail(c, OVP_ERR_BAD_ARGS, "ekf_update: empty system");
   if (rows > c->Rcap)
     return fail(c, OVP_ERR_CAPACITY, "ekf_update: %d rows exceed capacity %d (compress first, like the reference's callers)", rows, c->Rcap);
-  st = ensure_stage(c, (size_t)rows * n + 2 * rows);
-  if (st)
+  const size_t col = (size_t)rows * sizeof(double);
+  StageLayout L;
+  const size_t b_H = L.take(col * n), b_res = L.take(col), b_R = L.take(col);
+  if ((st = ensure_stage(c, L)))
     return st;
-  double *dH = c->d_stage, *dres = c->d_stage + (size_t)rows * n, *dR = dres + rows;
-  OVP_CUDA(cudaMemcpyAsync(dH, H, (size_t)rows * n * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(dres, res, (size_t)rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  if (Rdiag)
-    OVP_CUDA(cudaMemcpyAsync(dR, Rdiag, (size_t)rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  double *dH = (double *)(c->d_stage + b_H), *dres = (double *)(c->d_stage + b_res), *dR = (double *)(c->d_stage + b_R);
+  if ((st = stage_copy_in(c, dH, H, col * n)) || (st = stage_copy_in(c, dres, res, col)) || (Rdiag && (st = stage_copy_in(c, dR, Rdiag, col))))
+    return st;
   st = ekf_update_core(c, c->dcols, n, mv(dH, rows, 1), rows, dres, Rdiag ? dR : nullptr, -1.0, nullptr, nullptr);
   if (st)
     return st;
   return check_status_flags(c);
 }
 
-int ovp_marginalize(ovp_ctx *h, int handle) { return do_marginalize(&h->c, handle); }
+int ovp_marginalize(ovp_ctx *h, int handle) { return do_marginalize(ovp::enter(h), handle); }
 
 int ovp_clone(ovp_ctx *h, int handle, int *new_handle) {
   Ctx *c = ovp::enter(h);
@@ -241,7 +244,8 @@ int ovp_augment_clone(ovp_ctx *h, double timestamp, const double last_w[3], int 
     double dnc[6] = {last_w[0], last_w[1], last_w[2], c->h_val[(size_t)c->h_imu * OVP_VAL_STRIDE + 7],
                      c->h_val[(size_t)c->h_imu * OVP_VAL_STRIDE + 8], c->h_val[(size_t)c->h_imu * OVP_VAL_STRIDE + 9]};
     double *dd = c->dscal + 64;
-    OVP_CUDA(cudaMemcpyAsync(dd, dnc, sizeof(dnc), cudaMemcpyHostToDevice, c->stream));
+    if ((st = stage_copy_in(c, dd, dnc, sizeof(dnc))))
+      return st;
     int rows = c->N, newid = c->vars[nh].id, dtid = c->vars[c->h_dt].id;
     dt_col_kernel<<<(rows * 6 + 255) / 256, 256, 0, c->stream>>>(c->dP, c->ldP, rows, newid, dtid, dd);
     dt_row_kernel<<<(rows * 6 + 255) / 256, 256, 0, c->stream>>>(c->dP, c->ldP, rows, newid, dtid, dd);
@@ -322,7 +326,8 @@ int initialize_core(Ctx *c, int kind, int s, const double *value, const double *
     int st = ekf_update_core(c, d_cols, n, HupT, ru, d_resup, dR, -1.0, nullptr, c->dscal, false); // dry run: chi2 only (:464-475)
     if (st)
       return st;
-    OVP_CUDA(cudaMemcpyAsync(&chi2, c->dscal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    if ((st = stage_copy_out(c, &chi2, c->dscal, sizeof(double))))
+      return st;
     OVP_CUDA(cudaStreamSynchronize(c->stream));
   }
   int st = check_status_flags(c);
@@ -537,12 +542,19 @@ int ovp_merge_planes_and_marginalize(ovp_ctx *h, const int64_t *f2p_feat, const 
 // ---- stateless helpers -----------------------------------------------------------------------------------------------
 } // extern "C"
 namespace ovp {
-// get_feature_jacobian_full of ONE feature staged on the device in the layout StateHelper::initialize wants:
-// d_stage = [H_f (rows x hfc) | H_x (rows x hxc) | res (rows)], all with leading dimension `rows`.
+// get_feature_jacobian_full of ONE feature on the staging buffer, in the layout StateHelper::initialize wants:
+// W = [H_f (rows x hfc) | H_x (rows x hxc) | res (rows)], leading dimension `rows`, then the measurements' uv.
+struct FeatureJacobianStage {
+  int rows, hfc, hxc;
+  size_t b_W, b_uv; // byte offsets into c->d_stage
+  double *W(const Ctx *c) const { return (double *)(c->d_stage + b_W); }
+  double *Hx(const Ctx *c) const { return W(c) + (size_t)rows * hfc; }
+  double *res(const Ctx *c) const { return W(c) + (size_t)rows * (hfc + hxc); }
+};
 // plane_handle >= 0: plane in the state (its values come from the device tables); otherwise cp / cp_fej (may be null: no plane).
 static int stage_feature_jacobian(Ctx *c, int m, const int *clone_handles, const float *uv, const double *p_FinG, const double *p_FinG_fej,
                                   bool has_plane, int plane_handle, const double *cp, const double *cp_fej, double sigma_px, double sigma_c,
-                                  int *rows_out, int *hfc_out, int *hxc_out, int extra_hx_cols = 0) {
+                                  FeatureJacobianStage *j, int extra_hx_cols = 0) {
   if (m > 64) // a size argument, not a track a feature kernel holds
     return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full: m=%d not in 1..64", m);
   const int off[2] = {0, m};
@@ -555,17 +567,18 @@ static int stage_feature_jacobian(Ctx *c, int m, const int *clone_handles, const
   const int rows = has_plane ? 3 * m : 2 * m;
   const int hfc = 3 + ((has_plane && !in_state) ? 3 : 0);
   const int hxc = ncal + 6 * m + (in_state ? 3 : 0) + extra_hx_cols; // extra: zero columns appended for an anchor clone (anchors.cu)
-  size_t e = (size_t)rows * (hfc + hxc + 1) + 256;
-  st = ensure_stage(c, e);
-  if (st)
+  const size_t w_bytes = (size_t)rows * (hfc + hxc + 1) * sizeof(double), uv_bytes = (size_t)m * 2 * sizeof(float);
+  StageLayout L;
+  *j = {rows, hfc, hxc, L.take(w_bytes), L.take(uv_bytes)};
+  if ((st = ensure_stage(c, L)))
     return st;
-  OVP_CUDA(cudaMemsetAsync(c->d_stage, 0, e * sizeof(double), c->stream));
+  OVP_CUDA(cudaMemsetAsync(j->W(c), 0, w_bytes, c->stream));
   JacArgs a;
   a.m = m;
   int *dcl = c->dcols + (size_t)4 * c->Rcap;
-  float *duv = (float *)(c->d_stage + (size_t)rows * (hfc + hxc + 1));
-  OVP_CUDA(cudaMemcpyAsync(dcl, clone_handles, m * sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(duv, uv, 2 * m * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  float *duv = (float *)(c->d_stage + j->b_uv);
+  if ((st = stage_copy_in(c, dcl, clone_handles, m * sizeof(int))) || (st = stage_copy_in(c, duv, uv, uv_bytes)))
+    return st;
   a.clone_handles = dcl;
   a.uv = duv;
   for (int i = 0; i < 3; i++) {
@@ -586,17 +599,24 @@ static int stage_feature_jacobian(Ctx *c, int m, const int *clone_handles, const
   a.do_calib_intr = c->opt.do_calib_camera_intrinsics;
   a.white_px = 1.0 / sigma_px;
   a.white_c = 1.0 / sigma_c;
-  a.Hf = c->d_stage;
-  a.Hx = c->d_stage + (size_t)rows * hfc;
-  a.res = c->d_stage + (size_t)rows * (hfc + hxc);
+  a.Hf = j->W(c);
+  a.Hx = j->Hx(c);
+  a.res = j->res(c);
   a.rows = rows;
   a.hf_cols = hfc;
   a.hx_cols = hxc;
   jacobian_only_kernel<<<1, 64, 0, c->stream>>>(a);
   c->launches++;
-  *rows_out = rows;
-  *hfc_out = hfc;
-  *hxc_out = hxc;
+  return OVP_OK;
+}
+// the first hf_cols columns of H_f, then H_x and res of a staged feature Jacobian, to the host
+static int read_feature_jacobian(Ctx *c, const FeatureJacobianStage &j, int hf_cols, double *H_f, double *H_x, double *res) {
+  const size_t col = (size_t)j.rows * sizeof(double);
+  int st;
+  if ((st = stage_copy_out(c, H_f, j.W(c), col * hf_cols)) || (st = stage_copy_out(c, H_x, j.Hx(c), col * j.hxc)) ||
+      (st = stage_copy_out(c, res, j.res(c), col)))
+    return st;
+  OVP_CUDA(cudaStreamSynchronize(c->stream));
   return OVP_OK;
 }
 } // namespace ovp
@@ -677,21 +697,14 @@ int ovp_feature_jacobian_full(ovp_ctx *h, int m, const int *clone_handles, const
   Ctx *c = ovp::enter(h);
   const bool has_plane = planeid != 0;
   const bool in_state = has_plane && c->planes.count(planeid);
-  int rows, hfc, hxc;
+  FeatureJacobianStage j;
   int st = stage_feature_jacobian(c, m, clone_handles, uv, p_FinG, p_FinG_fej, has_plane, in_state ? c->planes[planeid] : -1, cp, cp_fej,
-                                  sigma_px, sigma_c, &rows, &hfc, &hxc);
-  if (st)
+                                  sigma_px, sigma_c, &j);
+  if (st || (st = read_feature_jacobian(c, j, j.hfc, H_f, H_x, res)))
     return st;
-  struct {
-    double *Hf, *Hx, *res;
-  } a = {c->d_stage, c->d_stage + (size_t)rows * hfc, c->d_stage + (size_t)rows * (hfc + hxc)};
-  OVP_CUDA(cudaMemcpyAsync(H_f, a.Hf, (size_t)rows * hfc * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(H_x, a.Hx, (size_t)rows * hxc * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(res, a.res, (size_t)rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  OVP_CUDA(cudaStreamSynchronize(c->stream));
-  *hf_cols = hfc;
-  *hx_cols = hxc;
-  *rows_out = rows;
+  *hf_cols = j.hfc;
+  *hx_cols = j.hxc;
+  *rows_out = j.rows;
   int no = 0;
   if (c->opt.do_calib_camera_pose)
     x_order[no++] = c->h_calib;
@@ -710,39 +723,36 @@ static int nullspace_common(Ctx *c, double *H_f, int hf_cols, double *H_x, int h
     return fail(c, OVP_ERR_BAD_ARGS, "nullspace_project: need rows >= H_f.cols() (assert, UpdaterHelper.cpp:518)");
   int ncp = H_cp ? 3 : 0;
   int ncols = hf_cols + hx_cols + ncp + 1;
-  int st = ensure_stage(c, (size_t)rows * ncols);
+  // W = [H_f | H_x | H_cp | res], leading dimension rows
+  const size_t col = (size_t)rows * sizeof(double);
+  StageLayout L;
+  const size_t b_W = L.take(col * ncols);
+  int st = ensure_stage(c, L);
   if (st)
     return st;
-  double *W = c->d_stage;
-  OVP_CUDA(cudaMemcpyAsync(W, H_f, (size_t)rows * hf_cols * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(W + (size_t)rows * hf_cols, H_x, (size_t)rows * hx_cols * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  if (H_cp)
-    OVP_CUDA(cudaMemcpyAsync(W + (size_t)rows * (hf_cols + hx_cols), H_cp, (size_t)rows * 3 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(W + (size_t)rows * (hf_cols + hx_cols + ncp), res, (size_t)rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  double *W = (double *)(c->d_stage + b_W), *Wx = W + (size_t)rows * hf_cols, *Wcp = Wx + (size_t)rows * hx_cols, *Wres = Wcp + (size_t)rows * ncp;
+  if ((st = stage_copy_in(c, W, H_f, col * hf_cols)) || (st = stage_copy_in(c, Wx, H_x, col * hx_cols)) ||
+      (H_cp && (st = stage_copy_in(c, Wcp, H_cp, col * 3))) || (st = stage_copy_in(c, Wres, res, col)))
+    return st;
   householder_cols_kernel<<<1, 256, 0, c->stream>>>(W, rows, rows, ncols, hf_cols);
   c->launches++;
   OVP_CUDA(cudaGetLastError());
   int ro = rows - hf_cols;
   // copy back rows [hf_cols, rows) compacted to ld = ro (none when H_f is square)
-  if (ro > 0) {
-    OVP_CUDA(cudaMemcpy2DAsync(H_x, (size_t)ro * sizeof(double), W + (size_t)rows * hf_cols + hf_cols, (size_t)rows * sizeof(double),
-                               (size_t)ro * sizeof(double), hx_cols, cudaMemcpyDeviceToHost, c->stream));
-    if (H_cp)
-      OVP_CUDA(cudaMemcpy2DAsync(H_cp, (size_t)ro * sizeof(double), W + (size_t)rows * (hf_cols + hx_cols) + hf_cols,
-                                 (size_t)rows * sizeof(double), (size_t)ro * sizeof(double), 3, cudaMemcpyDeviceToHost, c->stream));
-    OVP_CUDA(cudaMemcpyAsync(res, W + (size_t)rows * (hf_cols + hx_cols + ncp) + hf_cols, (size_t)ro * sizeof(double), cudaMemcpyDeviceToHost,
-                             c->stream));
-  }
+  const size_t rcol = (size_t)ro * sizeof(double);
+  if ((st = stage_copy2d_out(c, H_x, rcol, Wx + hf_cols, col, rcol, hx_cols)) ||
+      (H_cp && (st = stage_copy2d_out(c, H_cp, rcol, Wcp + hf_cols, col, rcol, 3))) || (st = stage_copy_out(c, res, Wres + hf_cols, rcol)))
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   *rows_out = ro;
   return OVP_OK;
 }
 int ovp_nullspace_project_inplace(ovp_ctx *h, double *H_f, int hf_cols, double *H_x, int hx_cols, double *res, int rows, int *rows_out) {
-  return nullspace_common(&h->c, H_f, hf_cols, H_x, hx_cols, nullptr, res, rows, rows_out);
+  return nullspace_common(ovp::enter(h), H_f, hf_cols, H_x, hx_cols, nullptr, res, rows, rows_out);
 }
 int ovp_plane_nullspace_project_inplace(ovp_ctx *h, double *H_f, int hf_cols, double *H_x, int hx_cols, double *H_cp, double *res, int rows,
                                         int *rows_out) {
-  return nullspace_common(&h->c, H_f, hf_cols, H_x, hx_cols, H_cp, res, rows, rows_out);
+  return nullspace_common(ovp::enter(h), H_f, hf_cols, H_x, hx_cols, H_cp, res, rows, rows_out);
 }
 
 static int compress_common(Ctx *c, double *H_x, int cols, double *H_cp, double *res, int rows, int *rows_out) {
@@ -757,22 +767,20 @@ static int compress_common(Ctx *c, double *H_x, int cols, double *H_cp, double *
     return fail(c, OVP_ERR_CAPACITY, "measurement_compress: %d rows exceed capacity %d", rows, c->max_meas_rows);
   int ld = (rows + 7) & ~7;
   launch_fill(c, c->dHs, (size_t)ld * nc1, 0.0);
-  OVP_CUDA(cudaMemcpy2DAsync(c->dHs, (size_t)ld * sizeof(double), H_x, (size_t)rows * sizeof(double), (size_t)rows * sizeof(double), cols,
-                             cudaMemcpyHostToDevice, c->stream));
-  if (H_cp)
-    OVP_CUDA(cudaMemcpy2DAsync(c->dHs + (size_t)ld * cols, (size_t)ld * sizeof(double), H_cp, (size_t)rows * sizeof(double),
-                               (size_t)rows * sizeof(double), 3, cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(c->dHs + (size_t)ld * (cols + ncp), res, (size_t)rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  int st = gram_of_stacked(c, rows, nc1, ld);
-  if (st)
+  const size_t col = (size_t)rows * sizeof(double), dcol = (size_t)ld * sizeof(double); // stacked [H_x | H_cp | res], leading dimension ld
+  int st;
+  if ((st = stage_copy2d_in(c, c->dHs, dcol, H_x, col, col, cols)) ||
+      (H_cp && (st = stage_copy2d_in(c, c->dHs + (size_t)ld * cols, dcol, H_cp, col, col, 3))) ||
+      (st = stage_copy_in(c, c->dHs + (size_t)ld * (cols + ncp), res, col)) || (st = gram_of_stacked(c, rows, nc1, ld)))
     return st;
   st = chol_partial(c, c->wsG.S, c->wsG.cap, nc1, cols, c->gram_tol);
   if (st)
     return st;
   // R = L[0:cols,0:cols]^T ; carried columns = L[cols.., 0:cols]^T
   std::vector<double> L((size_t)nc1 * cols);
-  OVP_CUDA(cudaMemcpy2DAsync(L.data(), (size_t)nc1 * sizeof(double), c->wsG.S, (size_t)c->wsG.cap * sizeof(double), (size_t)nc1 * sizeof(double),
-                             cols, cudaMemcpyDeviceToHost, c->stream));
+  if ((st = stage_copy2d_out(c, L.data(), (size_t)nc1 * sizeof(double), c->wsG.S, (size_t)c->wsG.cap * sizeof(double), (size_t)nc1 * sizeof(double),
+                             cols)))
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   const int r = cols; // min(rows, cols)
   for (int j = 0; j < cols; j++)
@@ -788,10 +796,10 @@ static int compress_common(Ctx *c, double *H_x, int cols, double *H_cp, double *
   return OVP_OK;
 }
 int ovp_measurement_compress_inplace(ovp_ctx *h, double *H_x, int cols, double *res, int rows, int *rows_out) {
-  return compress_common(&h->c, H_x, cols, nullptr, res, rows, rows_out);
+  return compress_common(ovp::enter(h), H_x, cols, nullptr, res, rows, rows_out);
 }
 int ovp_plane_measurement_compress_inplace(ovp_ctx *h, double *H_x, int cols, double *H_cp, double *res, int rows, int *rows_out) {
-  return compress_common(&h->c, H_x, cols, H_cp, res, rows, rows_out);
+  return compress_common(ovp::enter(h), H_x, cols, H_cp, res, rows, rows_out);
 }
 
 // ---- UpdaterMSCKF ------------------------------------------------------------------------------------------------------
@@ -862,7 +870,8 @@ int ovp_msckf_update_gathered(ovp_ctx *h, const double *d_blocks, int G, const i
   const int rows = G * n, nc1 = n + 1;
   if (rows > c->max_meas_rows || nc1 > c->Rcap)
     return fail(c, OVP_ERR_CAPACITY, "gathered system %d x %d exceeds capacity", rows, nc1);
-  OVP_CUDA(cudaMemcpyAsync(c->dcols, cols.data(), n * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  if ((st = stage_copy_in(c, c->dcols, cols.data(), n * sizeof(int))))
+    return st;
   int ld = (rows + 7) & ~7;
   launch_fill(c, c->dHs, (size_t)ld * nc1, 0.0);
   transpose_stack_kernel<<<c->num_sms * 4, 256, 0, c->stream>>>(d_blocks, G, n, c->dHs, ld);
@@ -1389,11 +1398,12 @@ int ovp_msckf_prepare_landmarks(ovp_ctx *h, const ovp_feature_batch *batch, cons
 int ovp_msckf_prepare(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updater_options *opt) {
   return ovp_msckf_prepare_landmarks(h, batch, nullptr, opt);
 }
-int ovp_msckf_launch(ovp_ctx *h) { return msckf_launch(&h->c); }
+int ovp_msckf_launch(ovp_ctx *h) { return msckf_launch(ovp::enter(h)); }
 int ovp_msckf_finish(ovp_ctx *h, int *feat_status, double *feat_chi2, int *plane_status, double *plane_chi2, int *hx_order, int *hx_order_n) {
+  Ctx *c = ovp::enter(h);
   if (hx_order_n)
     *hx_order_n = 0;
-  return msckf_finish(&h->c, feat_status, feat_chi2, plane_status, plane_chi2, hx_order, hx_order_n);
+  return msckf_finish(c, feat_status, feat_chi2, plane_status, plane_chi2, hx_order, hx_order_n);
 }
 
 int ovp_snapshot(ovp_ctx *h) {
@@ -1614,7 +1624,8 @@ int ovp_zupt_try_update(ovp_ctx *h, const ovp_zupt_options *zo, double timestamp
     return OVP_OK;
   }
   // accepted (:253-264): bias propagation, then the update, then move the state time forward
-  OVP_CUDA(cudaMemcpyAsync(c->dscal + 32, Qb, 6 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  if ((st = stage_copy_in(c, c->dscal + 32, Qb, sizeof(Qb))))
+    return st;
   add_diag6_kernel<<<1, 32, 0, c->stream>>>(c->dP, c->ldP, c->vars[c->h_imu].id + 9, c->dscal + 32);
   c->launches++;
   st = ovp_ekf_update(h, &c->h_imu, 1, H.data(), m, res.data(), Rd.data());
@@ -1655,9 +1666,9 @@ static int slam_delayed_init_impl(Ctx *c, int F, const int *meas_offset, const i
         ph = ip->second;
     }
     auto attempt = [&](const double *pf, int plane_h, int *acc, int *nh) -> int {
-      int rows, hfc, hxc;
+      FeatureJacobianStage j;
       int st = stage_feature_jacobian(c, m, cl, uv + 2 * (size_t)meas_offset[f], pf, pf, plane_h >= 0, plane_h, nullptr, nullptr,
-                                      opt->sigma_pix, c->opt.sigma_constraint, &rows, &hfc, &hxc);
+                                      opt->sigma_pix, c->opt.sigma_constraint, &j);
       if (st)
         return st;
       std::vector<int> xo;
@@ -1673,14 +1684,14 @@ static int slam_delayed_init_impl(Ctx *c, int F, const int *meas_offset, const i
       st = upload_cols(c, xo.data(), (int)xo.size(), 0, &n);
       if (st)
         return st;
-      if (n != hxc)
-        return fail(c, OVP_ERR_BAD_ARGS, "delayed_init: internal column mismatch %d vs %d", n, hxc);
+      if (n != j.hxc)
+        return fail(c, OVP_ERR_BAD_ARGS, "delayed_init: internal column mismatch %d vs %d", n, j.hxc);
       if (c->var_table_dirty) {
         st = upload_var_table(c);
         if (st)
           return st;
       }
-      return initialize_core(c, OVP_KIND_LANDMARK, 3, pf, pf, featid[f], c->dcols, n, c->d_stage, rows, rows, rows, 1.0, opt->chi2_multipler,
+      return initialize_core(c, OVP_KIND_LANDMARK, 3, pf, pf, featid[f], c->dcols, n, j.W(c), j.rows, j.rows, j.rows, 1.0, opt->chi2_multipler,
                              1, acc, nh);
     };
     int acc = 0, nh = -1;

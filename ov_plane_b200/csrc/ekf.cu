@@ -134,6 +134,46 @@ __global__ void diag_check_kernel(const double *P, int ld, int N, int *flag_out,
     atomicExch(flag_out, 1);
 }
 
+// The staging buffer grows on demand and is only replaced after the stream has drained (kernels in flight may still read it); snapshots,
+// profiling events and the prepared batch belong to other owners and are released in ovp_destroy.
+int ensure_stage(Ctx *c, const StageLayout &L) {
+  if (L.top <= c->d_stage_bytes)
+    return OVP_OK;
+  OVP_CUDA(cudaStreamSynchronize(c->stream));
+  if (c->d_stage)
+    cudaFree(c->d_stage);
+  c->d_stage = nullptr;
+  c->d_stage_bytes = 0;
+  size_t n = std::max<size_t>(L.top * 2, 1 << 19);
+  OVP_CUDA(cudaMalloc(&c->d_stage, n));
+  c->d_stage_bytes = n;
+  return OVP_OK;
+}
+
+static int counted_copy(Ctx *c, void *dst, size_t dpitch, const void *src, size_t spitch, size_t col_bytes, size_t cols, cudaMemcpyKind kind,
+                        int64_t *counter) {
+  if (col_bytes == 0 || cols == 0)
+    return OVP_OK;
+  if (cols == 1)
+    OVP_CUDA(cudaMemcpyAsync(dst, src, col_bytes, kind, c->stream));
+  else
+    OVP_CUDA(cudaMemcpy2DAsync(dst, dpitch, src, spitch, col_bytes, cols, kind, c->stream));
+  *counter += (int64_t)(col_bytes * cols);
+  return OVP_OK;
+}
+int stage_copy_in(Ctx *c, void *dst, const void *src, size_t bytes) {
+  return counted_copy(c, dst, bytes, src, bytes, bytes, 1, cudaMemcpyHostToDevice, &c->h2d_bytes);
+}
+int stage_copy_out(Ctx *c, void *dst, const void *src, size_t bytes) {
+  return counted_copy(c, dst, bytes, src, bytes, bytes, 1, cudaMemcpyDeviceToHost, &c->d2h_bytes);
+}
+int stage_copy2d_in(Ctx *c, void *dst, size_t dpitch, const void *src, size_t spitch, size_t col_bytes, size_t cols) {
+  return counted_copy(c, dst, dpitch, src, spitch, col_bytes, cols, cudaMemcpyHostToDevice, &c->h2d_bytes);
+}
+int stage_copy2d_out(Ctx *c, void *dst, size_t dpitch, const void *src, size_t spitch, size_t col_bytes, size_t cols) {
+  return counted_copy(c, dst, dpitch, src, spitch, col_bytes, cols, cudaMemcpyDeviceToHost, &c->d2h_bytes);
+}
+
 int upload_var_table(Ctx *c) {
   int nh = (int)c->vars.size();
   if (nh > c->max_handles)
@@ -144,9 +184,10 @@ int upload_var_table(Ctx *c) {
     sz[h] = c->vars[h].size;
     kd[h] = c->vars[h].kind;
   }
-  OVP_CUDA(cudaMemcpyAsync(c->d_var_id, id.data(), nh * sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(c->d_var_size, sz.data(), nh * sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(c->d_var_kind, kd.data(), nh * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  int st;
+  if ((st = stage_copy_in(c, c->d_var_id, id.data(), nh * sizeof(int))) || (st = stage_copy_in(c, c->d_var_size, sz.data(), nh * sizeof(int))) ||
+      (st = stage_copy_in(c, c->d_var_kind, kd.data(), nh * sizeof(int))))
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream)); // host vectors go out of scope
   c->var_table_dirty = false;
   return OVP_OK;
@@ -155,19 +196,19 @@ int upload_var_table(Ctx *c) {
 int sync_host_values(Ctx *c) {
   if (!c->host_values_stale)
     return OVP_OK;
-  size_t n = c->vars.size() * OVP_VAL_STRIDE;
-  OVP_CUDA(cudaMemcpyAsync(c->h_val.data(), c->d_val, n * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  int st = stage_copy_out(c, c->h_val.data(), c->d_val, c->vars.size() * OVP_VAL_STRIDE * sizeof(double));
+  if (st)
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
-  c->d2h_bytes += (int64_t)(n * sizeof(double));
   c->host_values_stale = false;
   return OVP_OK;
 }
 
 int push_host_values(Ctx *c, int h) {
-  OVP_CUDA(cudaMemcpyAsync(c->d_val + (size_t)h * OVP_VAL_STRIDE, c->h_val.data() + (size_t)h * OVP_VAL_STRIDE,
-                           OVP_VAL_STRIDE * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  OVP_CUDA(cudaMemcpyAsync(c->d_fej + (size_t)h * OVP_VAL_STRIDE, c->h_fej.data() + (size_t)h * OVP_VAL_STRIDE,
-                           OVP_VAL_STRIDE * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  const size_t at = (size_t)h * OVP_VAL_STRIDE, bytes = OVP_VAL_STRIDE * sizeof(double);
+  int st;
+  if ((st = stage_copy_in(c, c->d_val + at, c->h_val.data() + at, bytes)) || (st = stage_copy_in(c, c->d_fej + at, c->h_fej.data() + at, bytes)))
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   return OVP_OK;
 }
@@ -231,7 +272,9 @@ double chi2_q95(Ctx *c, int dof) {
 
 int check_status_flags(Ctx *c) {
   int f[2] = {0, 0};
-  OVP_CUDA(cudaMemcpyAsync(f, c->dflags, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  int st = stage_copy_out(c, f, c->dflags, sizeof(f));
+  if (st)
+    return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   if (f[0] || f[1]) {
     OVP_CUDA(cudaMemsetAsync(c->dflags, 0, 2 * sizeof(int), c->stream));

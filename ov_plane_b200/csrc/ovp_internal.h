@@ -115,9 +115,9 @@ struct Ctx {
   size_t d_batch_bytes = 0;
   void *h_pinned = nullptr;
   size_t h_pinned_bytes = 0;
-  // host staging for small dense transfers
-  double *d_stage = nullptr;
-  size_t d_stage_elems = 0;
+  // device side of the host <-> device transfers of the ABI entry points, laid out by a StageLayout (ensure_stage)
+  char *d_stage = nullptr;
+  size_t d_stage_bytes = 0;
 
   // Propagator
   double sigma_w = 1.6968e-04, sigma_wb = 1.9393e-05, sigma_a = 2.0000e-3, sigma_ab = 3.0000e-03;
@@ -272,4 +272,13 @@ struct StageLayout {
     return at;
   }
 };
+// c->d_stage grown to hold L's slices (its base is 16-byte aligned, like every slice)
+int ensure_stage(Ctx *c, const StageLayout &L);
+// Every host <-> device copy of the library goes through these: asynchronous on c->stream, counted in c->h2d_bytes / c->d2h_bytes
+// (ovp_transfer_bytes).  The 2D forms copy `cols` columns of col_bytes each between buffers with the given column pitches.  Nothing to
+// copy: no call.
+int stage_copy_in(Ctx *c, void *dst, const void *src, size_t bytes);
+int stage_copy_out(Ctx *c, void *dst, const void *src, size_t bytes);
+int stage_copy2d_in(Ctx *c, void *dst, size_t dpitch, const void *src, size_t spitch, size_t col_bytes, size_t cols);
+int stage_copy2d_out(Ctx *c, void *dst, size_t dpitch, const void *src, size_t spitch, size_t col_bytes, size_t cols);
 } // namespace ovp

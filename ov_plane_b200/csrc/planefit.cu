@@ -1045,22 +1045,6 @@ static TriOptions tri_options(const ovp_triangulation_options *q) {
   return {q->max_runs, q->init_lamda, q->max_lamda, q->min_dx, q->min_dcost, q->lam_mult, q->min_dist, q->max_dist, q->max_baseline, q->max_cond_number};
 }
 
-// counted copies between the host and slice `at` of the staging buffer d (nothing to copy: no call)
-static int stage_copy_in(Ctx *c, char *d, size_t at, const void *src, size_t bytes) {
-  if (bytes == 0)
-    return OVP_OK;
-  OVP_CUDA(cudaMemcpyAsync(d + at, src, bytes, cudaMemcpyHostToDevice, c->stream));
-  c->h2d_bytes += (int64_t)bytes;
-  return OVP_OK;
-}
-static int stage_copy_out(Ctx *c, void *dst, const char *d, size_t at, size_t bytes) {
-  if (bytes == 0)
-    return OVP_OK;
-  OVP_CUDA(cudaMemcpyAsync(dst, d + at, bytes, cudaMemcpyDeviceToHost, c->stream));
-  c->d2h_bytes += (int64_t)bytes;
-  return OVP_OK;
-}
-
 // camera pose table indexed by handle (R_GtoC: 9 doubles, p_CinG: 3) for the nh = c->vars.size() handles of the context
 struct PoseTable {
   size_t R, p;
@@ -1195,17 +1179,17 @@ int ovp_triangulate_features(ovp_ctx *h, int F, const int *meas_offset, const in
   const size_t b_off = L.take((size_t)(F + 1) * 4), b_cl = L.take((size_t)M * 4), b_uv = L.take((size_t)M * 8), b_pf = L.take((size_t)F * 24),
                b_st = L.take((size_t)F * 4);
   const PoseTable pose(L, (int)c->vars.size());
-  int st = ensure_stage(c, L.top / 8 + 8);
+  int st = ensure_stage(c, L);
   if (st)
     return st;
-  char *d = (char *)c->d_stage;
-  if ((st = stage_copy_in(c, d, b_off, meas_offset, (size_t)(F + 1) * 4)) || (st = stage_copy_in(c, d, b_cl, meas_clone, (size_t)M * 4)) ||
-      (st = stage_copy_in(c, d, b_uv, uv_norm, (size_t)M * 8)))
+  char *d = c->d_stage;
+  if ((st = stage_copy_in(c, d + b_off, meas_offset, (size_t)(F + 1) * 4)) || (st = stage_copy_in(c, d + b_cl, meas_clone, (size_t)M * 4)) ||
+      (st = stage_copy_in(c, d + b_uv, uv_norm, (size_t)M * 8)))
     return st;
   launch_cam_poses(c, d, pose);
   if ((st = launch_triangulate(c, F, (const int *)(d + b_off), (const int *)(d + b_cl), (const float *)(d + b_uv), tri_options(opt), d, pose,
                                (double *)(d + b_pf), (int *)(d + b_st))) ||
-      (st = stage_copy_out(c, p_FinG, d, b_pf, (size_t)F * 24)) || (st = stage_copy_out(c, status, d, b_st, (size_t)F * 4)))
+      (st = stage_copy_out(c, p_FinG, d + b_pf, (size_t)F * 24)) || (st = stage_copy_out(c, status, d + b_st, (size_t)F * 4)))
     return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   return OVP_OK;
@@ -1256,7 +1240,7 @@ int ovp_plane_fitting(ovp_ctx *h, int n_planes, const int *feat_offset, const do
   const size_t b_fo = L.take((size_t)(n_planes + 1) * 4), b_po = L.take((size_t)n_planes * 4), b_pm = L.take(plan.perms.size() * 4),
                b_pt = L.take((size_t)Ftot * 24), b_in_end = L.top;
   const RansacOut out(L, n_planes, Ftot);
-  int st = ensure_stage(c, L.top / 8 + 8);
+  int st = ensure_stage(c, L);
   if (st)
     return st;
   std::vector<char> hbuf(b_in_end);
@@ -1264,12 +1248,12 @@ int ovp_plane_fitting(ovp_ctx *h, int n_planes, const int *feat_offset, const do
   std::memcpy(hbuf.data() + b_po, plan.perm_off.data(), (size_t)n_planes * 4);
   std::memcpy(hbuf.data() + b_pm, plan.perms.data(), plan.perms.size() * 4);
   std::memcpy(hbuf.data() + b_pt, p_FinG, (size_t)Ftot * 24);
-  char *d = (char *)c->d_stage;
-  if ((st = stage_copy_in(c, d, 0, hbuf.data(), b_in_end)) ||
+  char *d = c->d_stage;
+  if ((st = stage_copy_in(c, d, hbuf.data(), b_in_end)) ||
       (st = launch_plane_ransac(c, n_planes, plan.Fmax, (const int *)(d + b_fo), (const double *)(d + b_pt), (const int *)(d + b_pm),
                                 (const int *)(d + b_po), opt->max_cond_number, opt->min_inlier_num, d, out)) ||
-      (st = stage_copy_out(c, status, d, out.status, (size_t)n_planes * 4)) || (st = stage_copy_out(c, abcd, d, out.abcd, (size_t)n_planes * 32)) ||
-      (st = stage_copy_out(c, inlier, d, out.inlier, (size_t)Ftot * 4)))
+      (st = stage_copy_out(c, status, d + out.status, (size_t)n_planes * 4)) || (st = stage_copy_out(c, abcd, d + out.abcd, (size_t)n_planes * 32)) ||
+      (st = stage_copy_out(c, inlier, d + out.inlier, (size_t)Ftot * 4)))
     return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream)); // hbuf is pageable: the H2D copy above has completed by now as well
   return OVP_OK;
@@ -1327,7 +1311,7 @@ int ovp_optimize_plane(ovp_ctx *h, int n_planes, const int *feat_offset, const i
                b_c0 = L.take((size_t)n_planes * 24), b_in_end = L.top;
   const PoseTable pose(L, (int)c->vars.size());
   const RefineOut out(L, n_planes, Ftot);
-  st = ensure_stage(c, L.top / 8 + 8);
+  st = ensure_stage(c, L);
   if (st)
     return st;
   std::vector<char> hbuf(b_in_end);
@@ -1340,16 +1324,16 @@ int ovp_optimize_plane(ovp_ctx *h, int n_planes, const int *feat_offset, const i
   std::memcpy(hbuf.data() + b_fx, fix_plane, (size_t)n_planes * 4);
   std::memcpy(hbuf.data() + b_p0, p_FinG, (size_t)Ftot * 24);
   std::memcpy(hbuf.data() + b_c0, cp_inG, (size_t)n_planes * 24);
-  char *d = (char *)c->d_stage;
-  if ((st = stage_copy_in(c, d, 0, hbuf.data(), b_in_end)))
+  char *d = c->d_stage;
+  if ((st = stage_copy_in(c, d, hbuf.data(), b_in_end)))
     return st;
   launch_cam_poses(c, d, pose);
   if ((st = launch_optimize_plane(c, n_planes, (const int *)(d + b_fo), (const int *)(d + b_mo), (const int *)(d + b_mc), (const float *)(d + b_uv),
                                   (const double *)(d + b_p0), (const double *)(d + b_c0), (const int *)(d + b_fx), opt->sigma_px_norm, opt->sigma_c,
                                   opt->max_num_iterations > 0 ? opt->max_num_iterations : 12, d, pose, out)) || // PlaneFitting.cpp:396
-      (st = stage_copy_out(c, p_FinG_out, d, out.p, (size_t)Ftot * 24)) || (st = stage_copy_out(c, cp_out, d, out.cp, (size_t)n_planes * 24)) ||
-      (st = stage_copy_out(c, inlier, d, out.inlier, (size_t)Ftot * 4)) || (st = stage_copy_out(c, status, d, out.status, (size_t)n_planes * 4)) ||
-      (info && (st = stage_copy_out(c, info, d, out.info, (size_t)n_planes * 40))))
+      (st = stage_copy_out(c, p_FinG_out, d + out.p, (size_t)Ftot * 24)) || (st = stage_copy_out(c, cp_out, d + out.cp, (size_t)n_planes * 24)) ||
+      (st = stage_copy_out(c, inlier, d + out.inlier, (size_t)Ftot * 4)) || (st = stage_copy_out(c, status, d + out.status, (size_t)n_planes * 4)) ||
+      (info && (st = stage_copy_out(c, info, d + out.info, (size_t)n_planes * 40))))
     return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
   return OVP_OK;
