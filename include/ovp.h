@@ -298,7 +298,9 @@ typedef struct ovp_triangulation_options {
 /* FeatureInitializer::single_triangulation + single_gaussnewton for F features at once, against the clone and extrinsics values
  * that live in the context: meas_offset / meas_clone as in ovp_feature_batch (measurements in time order: the anchor is the last
  * one), uv_norm = Feature::uvs_norm (undistorted normalised coordinates, 2 floats per measurement).  status[f] = 1: p_FinG[3f..]
- * is the refined position; 0: the reference would drop the feature (condition number, depth range, baseline ratio, NaN). */
+ * is the refined position; 0: the reference would drop the feature (condition number, depth range, baseline ratio, NaN).
+ * opt == NULL runs the defaults.  Refused with OVP_ERR_BAD_ARGS before anything is copied or launched: a null pointer, meas_offset not
+ * starting at 0 or decreasing (so no track reaches past meas_offset[F]), a measurement whose handle is not a clone. */
 int ovp_triangulate_features(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv_norm,
                              const ovp_triangulation_options *opt, double *p_FinG, int *status);
 

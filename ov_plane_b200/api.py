@@ -55,6 +55,20 @@ class FeatureTracks(C.Structure):
                 ("featid", C.c_void_p), ("planeid", C.c_void_p)]
 
 
+class TriangulationOptions(C.Structure):
+    """ovp_triangulation_options: ov_core's FeatureInitializerOptions (include/ovp.h)"""
+    _fields_ = [("max_runs", C.c_int), ("init_lamda", C.c_double), ("max_lamda", C.c_double), ("min_dx", C.c_double), ("min_dcost", C.c_double),
+                ("lam_mult", C.c_double), ("min_dist", C.c_double), ("max_dist", C.c_double), ("max_baseline", C.c_double),
+                ("max_cond_number", C.c_double)]
+
+
+def _tri_options(options):
+    """a TriangulationOptions from a dict of its fields (None: NULL, the library's defaults)"""
+    if options is None:
+        return None
+    return TriangulationOptions(**{k: (int if t is C.c_int else float)(options[k]) for k, t in TriangulationOptions._fields_})
+
+
 class PlaneInitOptions(C.Structure):
     _fields_ = [("sigma_pix", C.c_double), ("max_msckf_plane", C.c_int), ("plane_init_min_feat", C.c_int), ("plane_init_max_cond", C.c_double),
                 ("shuffle_kind", C.c_int), ("tri", C.c_void_p)]
@@ -415,9 +429,11 @@ class Context(object):
         self._ck(self.lib.ovp_plane_init(self.h, C.byref(fb), C.byref(uo), _p(ps), _p(nh)))
         return dict(plane_status=ps[:fb.nplanes], new_handles=nh[:fb.nplanes])
 
-    def plane_init_tracks(self, tracks, sigma_pix=1.0, max_msckf_plane=20, plane_init_min_feat=8, plane_init_max_cond=200.0, shuffle_kind=0):
+    def plane_init_tracks(self, tracks, sigma_pix=1.0, max_msckf_plane=20, plane_init_min_feat=8, plane_init_max_cond=200.0, shuffle_kind=0,
+                          tri_options=None):
         """UpdaterPlane::init_vio_plane end to end on raw tracks (dict: meas_offset, meas_clone, uv, uv_norm, featid, planeid; see
-        include/ovp.h ovp_plane_init_tracks).  Returns feat_status, p_FinG, plane_ids, plane_status, new_handles, cp."""
+        include/ovp.h ovp_plane_init_tracks).  tri_options: a dict of the TriangulationOptions fields, None for the defaults.  Returns
+        feat_status, p_FinG, plane_ids, plane_status, new_handles, cp."""
         mo, mc = _i32(tracks["meas_offset"]), _i32(tracks["meas_clone"])
         uv = np.ascontiguousarray(tracks["uv"], dtype=np.float32)
         uvn = np.ascontiguousarray(tracks["uv_norm"], dtype=np.float32)
@@ -425,7 +441,9 @@ class Context(object):
         pid = np.ascontiguousarray(tracks["planeid"], dtype=np.int64)
         F = len(mo) - 1
         t = FeatureTracks(F, mo.ctypes.data, mc.ctypes.data, uv.ctypes.data, uvn.ctypes.data, fid.ctypes.data, pid.ctypes.data)
-        o = PlaneInitOptions(float(sigma_pix), int(max_msckf_plane), int(plane_init_min_feat), float(plane_init_max_cond), int(shuffle_kind), None)
+        tri = _tri_options(tri_options)
+        o = PlaneInitOptions(float(sigma_pix), int(max_msckf_plane), int(plane_init_min_feat), float(plane_init_max_cond), int(shuffle_kind),
+                             C.cast(C.pointer(tri), C.c_void_p) if tri is not None else None)
         n = max(1, F)
         fs, pf, npl = np.zeros(n, dtype=np.int32), np.zeros((n, 3)), C.c_int(0)
         pids, ps, nh, cp = np.zeros(n, dtype=np.int64), np.zeros(n, dtype=np.int32), np.zeros(n, dtype=np.int32), np.zeros((n, 3))
@@ -518,12 +536,14 @@ class Context(object):
         self._ck(self.lib.ovp_propagator_feed_imu(self.h, C.c_double(t), _p(w), _p(a)))
 
     # ---- FeatureInitializer (triangulation, the step before the update path) ----
-    def triangulate_features(self, meas_offset, meas_clone, uv_norm):
+    def triangulate_features(self, meas_offset, meas_clone, uv_norm, options=None):
+        """options: a dict of the TriangulationOptions fields, None for the defaults"""
         mo, mc = _i32(meas_offset), _i32(meas_clone)
         uvn = np.ascontiguousarray(uv_norm, dtype=np.float32)
         F = len(mo) - 1
         pf, st = np.zeros((max(1, F), 3)), np.zeros(max(1, F), dtype=np.int32)
-        self._ck(self.lib.ovp_triangulate_features(self.h, F, _p(mo), _p(mc), _p(uvn), None, _p(pf), _p(st)))
+        tri = _tri_options(options)
+        self._ck(self.lib.ovp_triangulate_features(self.h, F, _p(mo), _p(mc), _p(uvn), C.byref(tri) if tri is not None else None, _p(pf), _p(st)))
         return pf[:F], st[:F]
 
     # ---- PlaneFitting (plane hypothesis + refinement, the step before the plane Jacobians) ----

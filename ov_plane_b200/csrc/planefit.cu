@@ -1165,6 +1165,12 @@ int ovp_triangulate_features(ovp_ctx *h, int F, const int *meas_offset, const in
     return OVP_OK;
   if (!meas_offset || !meas_clone || !uv_norm || !p_FinG || !status)
     return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: null argument");
+  // a track must not reach past the M = meas_offset[F] measurements that are staged
+  if (meas_offset[0] != 0)
+    return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: meas_offset must start at 0");
+  for (int f = 0; f < F; f++)
+    if (meas_offset[f + 1] < meas_offset[f])
+      return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: meas_offset is not non-decreasing at feature %d", f);
   const int M = meas_offset[F];
   for (int k = 0; k < M; k++)
     if (!is_clone(c, meas_clone[k], true))

@@ -16,7 +16,8 @@ def test_triangulation_matches_the_oracle(name, chi2_table):
     ctx, orc, chg, cho = make_pair(S, chi2_table)
     cam = S.intr_value
     uvn = np.array([vio_sim.undistort(cam, uv.astype(np.float64)) for uv in S.uv], dtype=np.float32)  # Feature::uvs_norm
-    # three degenerate tracks: two identical bearings (no parallax), a point behind the cameras, a far point
+    # one degenerate track: identical bearings (no parallax).  A point behind the cameras, a far point and every other rejection rule,
+    # on both sides of its threshold, are in tests/test_gpu_triangulation_reference.py
     uvn = uvn.copy()
     a, b = S.meas_offset[0], S.meas_offset[1]
     uvn[a:b] = uvn[a]
