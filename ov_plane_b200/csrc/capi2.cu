@@ -803,7 +803,7 @@ int ovp_plane_measurement_compress_inplace(ovp_ctx *h, double *H_x, int cols, do
 }
 
 // ---- UpdaterMSCKF ------------------------------------------------------------------------------------------------------
-// an empty landmark list is the plain update (same plan, same signature)
+// an empty landmark list is the plain update (same plan, same key)
 static const MsckfExtra *landmark_extra(const ovp_plane_landmarks *lm, MsckfExtra &ex) {
   if (!lm || lm->n == 0)
     return nullptr;
@@ -1658,13 +1658,7 @@ static int slam_delayed_init_impl(Ctx *c, int F, const int *meas_offset, const i
     const int *cl = meas_clone + meas_offset[f];
     if (c->slam.count(featid[f]))
       return fail(c, OVP_ERR_ALREADY_IN_STATE, "delayed_init: feature %lld already has a landmark", (long long)featid[f]);
-    int ph = -1;
-    if (use_plane && planeid && planeid[f] != 0) {
-      auto ip = c->planes.find(planeid[f]);
-      auto is = c->slam_to_plane.find(featid[f]);
-      if (ip != c->planes.end() && (is == c->slam_to_plane.end() || is->second != 0))
-        ph = ip->second;
-    }
+    const int ph = slam_plane_of(c, featid[f], planeid ? planeid[f] : 0, use_plane);
     auto attempt = [&](const double *pf, int plane_h, int *acc, int *nh) -> int {
       FeatureJacobianStage j;
       int st = stage_feature_jacobian(c, m, cl, uv + 2 * (size_t)meas_offset[f], pf, pf, plane_h >= 0, plane_h, nullptr, nullptr,

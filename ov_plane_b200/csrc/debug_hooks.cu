@@ -214,14 +214,14 @@ extern "C" int ovp_debug_chol_solve(ovp_ctx *h, const double *A, int n, int npiv
 }
 
 // Test hook (tests/test_gpu_numerics.py): on != 0 sends every later MSCKF batch of this context through the one-block-per-feature kernel
-// and the dense stacked system, whatever its longest track; the plan signature includes the setting.  Not part of the ABI in include/ovp.h.
+// and the dense stacked system, whatever its longest track; the plan key includes the setting.  Not part of the ABI in include/ovp.h.
 extern "C" int ovp_debug_force_dense_features(ovp_ctx *h, int on) {
   h->c.force_dense_features = on != 0;
   return OVP_OK;
 }
 
 // Test hook (tests/test_gpu_fused_products.py): on != 0 sends every later compressed update of this context through the factorisation
-// and two GEMM launches for M and S, instead of the factorisation that forms them; the plan signature includes the setting.  Not part of
+// and two GEMM launches for M and S, instead of the factorisation that forms them; the plan key includes the setting.  Not part of
 // the ABI in include/ovp.h.
 extern "C" int ovp_debug_unfused_update_products(ovp_ctx *h, int on) {
   h->c.unfused_update_products = on != 0;
@@ -294,7 +294,7 @@ static int debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, const ovp_pl
   int st = msckf_prepare(c, b, opt, lm && lm->n > 0 ? &ex : nullptr);
   if (st)
     return st;
-  Prepared &P = *(Prepared *)c->prep;
+  Prepared &P = *c->prep;
   const size_t nraw = (size_t)3 * OVP_RAW_ROW * std::max(P.M, 1);
   double *draw = nullptr;
   if (raw_out) {
@@ -307,7 +307,6 @@ static int debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, const ovp_pl
   st = msckf_launch_body(c, true);
   c->dbg_raw = nullptr;
   c->dbg_gram_stop = false;
-  P.valid = false; // the next update prepares its batch again (this one stopped half way)
   auto run = [&]() -> int {
     if (st)
       return st;
@@ -340,6 +339,7 @@ static int debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, const ovp_pl
     return OVP_OK;
   };
   st = run();
+  free_prepared(c); // the next update prepares its batch again (this one stopped half way)
   if (draw)
     cudaFree(draw);
   return st;

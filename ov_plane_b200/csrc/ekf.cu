@@ -226,7 +226,7 @@ __global__ void zero_band_kernel(double *P, int ld, int N, int s) {
 // Handles are slots of the variable table.  A marginalised variable's slot goes to a FIFO free list and is handed out again once
 // OVP_HANDLE_REUSE_LAG newer slots have been freed (a stale handle held by the caller keeps failing with NOT_IN_STATE for a while
 // instead of silently naming a new variable), so the table - and every O(table) pass: finish_update_kernel, upload_var_table,
-// sync_host_values, the plan signature - stays the size of the live state instead of growing by one clone per camera frame.
+// sync_host_values, the plan key - stays the size of the live state instead of growing by one clone per camera frame.
 #define OVP_HANDLE_REUSE_LAG 64
 int state_append_variable(Ctx *c, Var v, const double *value, const double *fej, int *handle) {
   int st = sync_host_values(c);

@@ -35,6 +35,8 @@ struct DenseWs {
   double *S = nullptr; // cap x cap (Gram / S, factored in place to lower L)
 };
 
+struct Prepared; // the plan of the last prepared MSCKF batch (features_host.inc)
+
 struct Ctx {
   int device = 0;
   int num_sms = 0; // SMs of the device: grid sizes of the grid-stride kernels and the tile / split-K choices scale with it
@@ -134,7 +136,7 @@ struct Ctx {
   cudaEvent_t ev[8];
   double last_ms[4] = {0, 0, 0, 0};
   // prepared feature batch (features_host.inc), byte counters of the host<->device copies this ctx issued
-  void *prep = nullptr;
+  Prepared *prep = nullptr;
   int64_t h2d_bytes = 0, d2h_bytes = 0;
   // snapshot of (P, values, fej) for repeatable benchmarking
   double *snapP = nullptr, *snap_val = nullptr, *snap_fej = nullptr;
