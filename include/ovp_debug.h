@@ -7,7 +7,8 @@
  * update products formed inside the Gram factorisation and run the update both with and without them, let
  * tests/test_gpu_compression.py check the compressed update's Gram matrix, zero-pivot rule and innovation gate element by element, and
  * let tests/test_gpu_feature_gate.py check the per-feature chi2 gates of the MSCKF point and SLAM feature kernels against long-double
- * references on the raw rows those kernels built. */
+ * references on the raw rows those kernels built, and let tests/test_gpu_plane_update_reference.py check the plane updates and plane
+ * initialisation, direct and compressed, against long-double references on the plan's raw rows or Gram matrix. */
 #ifndef OVP_DEBUG_H
 #define OVP_DEBUG_H
 #include "ovp.h"
@@ -61,7 +62,9 @@ int ovp_debug_chol_products(ovp_ctx *ctx, const double *G, int nc, int npiv, dou
  * per-feature status words after the plan's feature kernel (point plan: 1 accepted, 0 rejected by the gate).  raw_out (NULL, or 72
  * doubles per measurement of the batch): the raw whitened rows the feature kernel built, per measurement 3 rows of 24 doubles: the two
  * bearing rows [0,3) H_f, [3,9) H_clone, [9, 9 + ncal) calibration, [23] r, then (plane plans) the point-on-plane row [0,3) H_f,
- * [9,12) H_cp, [23] r.  A plan that updates without compression has no Gram matrix: OVP_ERR_BAD_ARGS. */
+ * [9,12) H_cp, [23] r.  A plan that updates without compression (the direct form) has no Gram matrix: the call stops after that plan's
+ * feature kernel, before its update, and returns OVP_OK with info[0] = 0 and info[5] = 0 (the direct form always runs the
+ * one-block-per-feature kernel); G_out is left as passed, and raw_out holds the rows the update would have stacked. */
 int ovp_debug_msckf_gram(ovp_ctx *ctx, const ovp_feature_batch *b, const ovp_updater_options *opt, int gcap, double *G_out, int *info,
                          int *cols_out, int *sel_out, int *feat_status, double *feat_chi2, double *raw_out);
 /* the same for ovp_msckf_update_landmarks: a plane plan's G also holds its landmark members' rows, their 3 columns each after the batch

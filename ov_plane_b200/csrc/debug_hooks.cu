@@ -280,8 +280,9 @@ extern "C" int ovp_debug_chol_products(ovp_ctx *h, const double *G, int nc, int 
 // [4] selected features nsel, [5] CTA-per-feature path, [6] plane slot, [7] plane in the state.  cols_out (gcap): compact column -> state
 // index of the x columns; sel_out (F): the plan's features; feat_status / feat_chi2 (F): the per-feature status words after the plan's
 // feature kernel.  raw_out (optional, 3 * OVP_RAW_ROW doubles per measurement, OVP_RAW_ROW in features.cu): the raw whitened rows the
-// feature kernel built.  A plan that goes straight into the update (no compression) has no Gram matrix: OVP_ERR_BAD_ARGS.  Not part of
-// the ABI in include/ovp.h.
+// feature kernel built.  A plan that goes straight into the update (no compression) has no Gram matrix: it stops after its feature
+// kernel, without updating, with info[0] = 0, info[5] = 0 and G_out untouched; raw_out holds its rows (tests/test_gpu_plane_update_reference.py).
+// Not part of the ABI in include/ovp.h.
 // ovp_debug_msckf_gram_landmarks: the same with the landmark members of ovp_msckf_update_landmarks (their columns follow the x columns
 // of the batch features, ncx counts them).
 static int debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, const ovp_plane_landmarks *lm, const ovp_updater_options *opt, int gcap,
@@ -312,20 +313,23 @@ static int debug_msckf_gram(ovp_ctx *h, const ovp_feature_batch *b, const ovp_pl
       return st;
     OVP_CUDA(cudaStreamSynchronize(c->stream));
     if (c->dbg_gram_plan < 0)
-      return fail(c, OVP_ERR_BAD_ARGS, "debug_msckf_gram: the first plan goes straight into the update, without a Gram matrix");
+      return fail(c, OVP_ERR_BAD_ARGS, "debug_msckf_gram: the batch has no plan with features");
     const UpdatePlan &pl = P.plans[c->dbg_gram_plan];
     const int ncx = pl.nx(), nc1 = pl.is_point ? ncx + 1 : ncx + 4;
     if (nc1 > gcap)
       return fail(c, OVP_ERR_CAPACITY, "debug_msckf_gram: %d columns, room for %d", nc1, gcap);
     const int ncal = (c->opt.do_calib_camera_pose ? 6 : 0) + (c->opt.do_calib_camera_intrinsics ? 8 : 0);
-    const int v[8] = {nc1, ncal, ncx, pl.is_point ? 1 : 0, (int)pl.feats.size(), P.fast ? 1 : 0, pl.plane_slot, pl.in_state ? 1 : 0};
+    // a plan that goes straight into the update has no Gram matrix: nc1 is reported as 0 and G_out is left as passed
+    const int v[8] = {pl.direct ? 0 : nc1, ncal, ncx, pl.is_point ? 1 : 0, (int)pl.feats.size(), P.fast && !pl.direct ? 1 : 0, pl.plane_slot,
+                      pl.in_state ? 1 : 0};
     std::memcpy(info, v, sizeof(v));
     std::memcpy(cols_out, pl.cols.data(), pl.cols.size() * sizeof(int));
     for (size_t k = 0; k < pl.lm_handle.size(); k++)
       for (int j = 0; j < 3; j++)
         cols_out[pl.cols.size() + 3 * k + j] = c->vars[pl.lm_handle[k]].id + j;
     std::memcpy(sel_out, pl.feats.data(), pl.feats.size() * sizeof(int));
-    OVP_CUDA(cudaMemcpy2DAsync(G_out, (size_t)nc1 * sizeof(double), c->wsG.S, (size_t)c->wsG.cap * sizeof(double), (size_t)nc1 * sizeof(double),
+    if (!pl.direct)
+      OVP_CUDA(cudaMemcpy2DAsync(G_out, (size_t)nc1 * sizeof(double), c->wsG.S, (size_t)c->wsG.cap * sizeof(double), (size_t)nc1 * sizeof(double),
                                nc1, cudaMemcpyDeviceToHost, c->stream));
     if (raw_out)
       OVP_CUDA(cudaMemcpyAsync(raw_out, draw, nraw * sizeof(double), cudaMemcpyDeviceToHost, c->stream));

@@ -297,8 +297,23 @@ int join_side_stream(Ctx *c) {
   return OVP_OK;
 }
 
+// flag &= (some feat_flag[i] == 1): one block
+__global__ void any_accepted_kernel(int *flag, const int *feat_flag, int n) {
+  __shared__ int any;
+  if (threadIdx.x == 0)
+    any = 0;
+  __syncthreads();
+  for (int i = threadIdx.x; i < n; i += blockDim.x)
+    if (feat_flag[i] == 1)
+      any = 1;
+  __syncthreads();
+  if (threadIdx.x == 0 && !any)
+    *flag = 0;
+}
+
 int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const double *d_z, const double *d_Rdiag, double gate_thresh,
-                    int *d_gate_flag, double *d_chi2, bool apply, int zstride, bool defer_join, bool ht_lower, bool products_done) {
+                    int *d_gate_flag, double *d_chi2, bool apply, int zstride, bool defer_join, bool ht_lower, bool products_done,
+                    const int *feat_flag, int nfeat) {
   if (rr <= 0 || nc <= 0)
     return OVP_OK;
   {
@@ -342,6 +357,10 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
   }
   if (!apply)
     return OVP_OK;
+  if (feat_flag) {
+    any_accepted_kernel<<<1, 256, 0, c->stream>>>(flag, feat_flag, nfeat);
+    c->launches++;
+  }
   // 6. P -= Y Y^T (lower tiles, mirrored) and the negative-diagonal check (StateHelper.cpp:176-187)  [skipped on the device when the gate
   //    failed].  Nothing downstream needs the new P before the next update's M = P[:, ids] H^T (or a point-feature gate), so this branch
   //    runs on the side stream, in parallel with step 7 and with whatever the caller enqueues next on the main stream.
@@ -379,7 +398,7 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
 }
 
 int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, double gate_thresh, int *d_gate_flag, double *d_chi2,
-                       bool defer_join) {
+                       bool defer_join, const int *feat_flag, int nfeat) {
   const int nc1 = nc + 1;
   const MatView L = mv(c->wsG.S, c->wsG.cap);
   const double *z = c->wsG.S + nc; // row nc of the factor, read in place (stride wsG.cap)
@@ -399,7 +418,8 @@ int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, 
     if (st)
       return st;
   }
-  return ekf_update_core(c, d_cols, nc, L, npiv, z, nullptr, gate_thresh, d_gate_flag, d_chi2, true, c->wsG.cap, defer_join, true, fused);
+  return ekf_update_core(c, d_cols, nc, L, npiv, z, nullptr, gate_thresh, d_gate_flag, d_chi2, true, c->wsG.cap, defer_join, true, fused,
+                         feat_flag, nfeat);
 }
 
 } // namespace ovp

@@ -209,13 +209,15 @@ void launch_fill(Ctx *c, double *p, size_t n, double v);
 // it on the device and the update is skipped when larger (flag written to d_gate_flag, chi2 to d_chi2).  ht_lower: HT(k, j) == 0 for k < j
 // (HT is the lower Cholesky factor of the compression) - the two products skip the structural zeros.
 // products_done: M = P[:, cols] HT (in dM) and S = HT^T M[cols, :] + R (in wsS) are already formed; steps 1-2 are skipped.
+// feat_flag (nfeat status words, or nullptr): the update is also skipped on the device when none of them is 1 (a point update none of
+// whose features passed its gate leaves the state untouched, UpdaterMSCKF.cpp:796-807).
 int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const double *d_z, const double *d_Rdiag, double gate_thresh,
                     int *d_gate_flag, double *d_chi2, bool apply = true, int zstride = 1, bool defer_join = false, bool ht_lower = false,
-                    bool products_done = false);
+                    bool products_done = false, const int *feat_flag = nullptr, int nfeat = 0);
 // The compressed update: factor the Gram matrix in wsG (nc + 1 columns, z last; pivots on the leading npiv) and update with H^T = L
 // (rows [0, nc)), z = row nc of the factor, R = I.  The factorisation launch also forms M and S.
 int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, double gate_thresh, int *d_gate_flag, double *d_chi2,
-                       bool defer_join);
+                       bool defer_join, const int *feat_flag = nullptr, int nfeat = 0);
 int join_side_stream(Ctx *c); // make the main stream wait for the side stream's covariance downdate (no-op when nothing is pending)
 int upload_var_table(Ctx *c);
 int sync_host_values(Ctx *c);
