@@ -76,44 +76,68 @@ void UpdaterSLAM::update(std::shared_ptr<State> state, std::vector<std::shared_p
 
 void UpdaterSLAM::delayed_init(std::shared_ptr<State> state, std::vector<std::shared_ptr<ov_core::Feature>> &feature_vec,
                                const std::map<size_t, size_t> &feat2plane) {
-  if (feature_vec.empty())
-    return;
-  // triangulation on the device (:118-160), failures leave
-  Flat tri;
+  // ArUco features (featid < max_aruco_features) need UpdaterSLAM's separate ArUco options, which the library does not take: they are left
+  // in feature_vec as they came, not initialised (use_aruco is false in every shipped config, so none arrive there)
+  std::vector<std::shared_ptr<ov_core::Feature>> aruco, slam;
   for (auto &f : feature_vec)
-    tri.append(state, *f, feat2plane);
-  std::vector<double> p(3 * feature_vec.size());
-  std::vector<int> ok(feature_vec.size());
-  ck(state->ctx, ovp_triangulate_features(state->ctx, (int)feature_vec.size(), tri.meas_offset.data(), tri.meas_clone.data(), tri.uvn.data(), nullptr,
-                                          p.data(), ok.data()));
-  Flat fl;
-  std::vector<std::shared_ptr<ov_core::Feature>> kept;
-  for (size_t i = 0; i < feature_vec.size(); i++) {
-    if (!ok[i]) {
-      feature_vec[i]->to_delete = true;
-      continue;
-    }
-    for (int k = 0; k < 3; k++)
-      feature_vec[i]->p_FinG(k) = p[3 * i + k];
-    fl.append(state, *feature_vec[i], feat2plane);
-    kept.push_back(feature_vec[i]);
-  }
-  if (kept.empty())
+    ((int)f->featid < state->_options.max_aruco_features ? aruco : slam).push_back(f);
+  feature_vec.swap(slam);
+  if (feature_vec.empty()) {
+    feature_vec.swap(aruco);
     return;
-  ovp_updater_options uo = {_options_slam.sigma_pix, _options_slam.chi2_multipler};
-  std::vector<int> st(kept.size()), nh(kept.size());
-  ck(state->ctx, ovp_slam_delayed_init(state->ctx, (int)kept.size(), fl.meas_offset.data(), fl.meas_clone.data(), fl.uv.data(), fl.p.data(), fl.p.data(),
-                                       fl.featid.data(), fl.planeid.data(), &uo, state->_options.use_plane_constraint_slamu ? 1 : 0, st.data(), nh.data()));
-  for (size_t i = 0; i < kept.size(); i++) {
-    kept[i]->to_delete = true;
-    if (st[i] == 0)
-      continue;
-    auto landmark = std::make_shared<ov_type::Landmark>(3); // _features_SLAM.insert (:338-339); values are refreshed from the device
-    landmark->_featid = kept[i]->featid;
-    state->_features_SLAM.insert({kept[i]->featid, landmark});
-    state->handle[landmark.get()] = nh[i];
-    state->by_handle[nh[i]] = landmark;
   }
+  // :77-103 clean every track against the clone times
+  std::vector<double> clonetimes;
+  for (const auto &clone_imu : state->_clones_IMU)
+    clonetimes.emplace_back(clone_imu.first);
+  for (auto &f : feature_vec)
+    f->clean_old_measurements(clonetimes);
+  // :106-364 in one call: triangulation, the refinement onto in-state planes, the initialisation with its chi2 fallback
+  Flat fl;
+  for (auto &f : feature_vec)
+    fl.append(state, *f, feat2plane);
+  ovp_feature_tracks t;
+  t.F = (int)feature_vec.size();
+  t.meas_offset = fl.meas_offset.data();
+  t.meas_clone = fl.meas_clone.data();
+  t.uv = fl.uv.data();
+  t.uv_norm = fl.uvn.data();
+  t.featid = fl.featid.data();
+  t.planeid = fl.planeid.data();
+  ovp_slam_init_options o;
+  o.sigma_pix = _options_slam.sigma_pix;
+  o.chi2_multipler = _options_slam.chi2_multipler;
+  o.use_plane_constraint = (state->_options.use_plane_constraint && state->_options.use_plane_constraint_slamd) ? 1 : 0;
+  o.use_refine_plane_feat = state->_options.use_refine_plane_feat ? 1 : 0;
+  o.tri = nullptr; // FeatureInitializerOptions defaults
+  const size_t F = feature_vec.size();
+  std::vector<int> feat_status(F), new_handles(F);
+  std::vector<double> p_FinG(3 * F);
+  ck(state->ctx, ovp_slam_delayed_init_tracks(state->ctx, &t, &o, feat_status.data(), nullptr, p_FinG.data(), new_handles.data()));
+  std::vector<std::shared_ptr<ov_core::Feature>> kept(aruco);
+  for (size_t i = 0; i < F; i++) {
+    auto &f = feature_vec[i];
+    f->to_delete = true; // every feature of the call (:98, :190, :306-361)
+    for (int k = 0; k < 3; k++)
+      f->p_FinG(k) = p_FinG[3 * i + k];
+    const int64_t s2p = ovp_slam_plane_of(state->ctx, (int64_t)f->featid); // written by the refinement and the initialisation
+    if (s2p >= 0)
+      state->_features_SLAM_to_PLANE[f->featid] = (size_t)s2p;
+    if (feat_status[i] <= 0)
+      continue; // erased from feature_vec
+    // :305, :352 register the landmark with the value and first estimate the device holds
+    auto landmark = std::make_shared<ov_type::Landmark>(3);
+    Eigen::MatrixXd value(3, 1), fej(3, 1);
+    ck(state->ctx, ovp_var_get(state->ctx, new_handles[i], value.data(), fej.data()));
+    landmark->_featid = f->featid;
+    landmark->set_value(value);
+    landmark->set_fej(fej);
+    state->_features_SLAM.insert({f->featid, landmark});
+    state->handle[landmark.get()] = new_handles[i];
+    state->by_handle[new_handles[i]] = landmark;
+    kept.push_back(f);
+  }
+  feature_vec.swap(kept);
 }
 
 void UpdaterSLAM::change_anchors(std::shared_ptr<State> state) { ck(state->ctx, ovp_slam_change_anchors(state->ctx, nullptr)); }

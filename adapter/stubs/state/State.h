@@ -10,9 +10,11 @@
 namespace ov_plane {
 struct StateOptions {
   int max_clone_size = 11;
+  int max_aruco_features = 1024;
   bool do_calib_camera_timeoffset = false;
   // StateOptions.h:96-150 (plane options the updaters read)
-  bool use_plane_constraint = true, use_plane_constraint_msckf = true, use_plane_constraint_slamu = true, use_refine_plane_feat = true;
+  bool use_plane_constraint = true, use_plane_constraint_msckf = true, use_plane_constraint_slamu = true,
+       use_plane_constraint_slamd = true, use_refine_plane_feat = true;
   double sigma_constraint = 0.01;
   int plane_msckf_min_feat = 20;
   double plane_msckf_max_cond = 100.0;

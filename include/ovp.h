@@ -380,6 +380,40 @@ typedef struct ovp_plane_init_options {
 int ovp_plane_init_tracks(ovp_ctx *ctx, const ovp_feature_tracks *t, const ovp_plane_init_options *opt, int *feat_status, double *p_FinG_out,
                           int *n_planes, int64_t *plane_ids, int *plane_status, int *new_handles, double *cp_out);
 
+/* ---- UpdaterSLAM::delayed_init end to end (UpdaterSLAM.cpp:66-374): new SLAM landmarks from raw feature tracks ---------------------------- */
+typedef struct ovp_slam_init_options {
+  double sigma_pix;                     /* UpdaterOptions::sigma_pix of the SLAM updater */
+  double chi2_multipler;                /* UpdaterOptions::chi2_multipler of the SLAM updater */
+  int use_plane_constraint;             /* StateOptions::use_plane_constraint && use_plane_constraint_slamd */
+  int use_refine_plane_feat;            /* StateOptions::use_refine_plane_feat */
+  const ovp_triangulation_options *tri; /* NULL = OpenVINS defaults */
+} ovp_slam_init_options;
+/* Longest track ovp_slam_delayed_init_tracks takes: the limit of a single feature's Jacobian (triangulation and refinement have none) */
+#define OVP_SLAM_INIT_MAX_TRACK 64
+/* Tracks as ovp_plane_init_tracks takes them (cleaned against the clone times; uv for the Jacobians, uv_norm for triangulation and
+ * refinement).  In the reference's order: a track with fewer than two measurements is erased; the others are triangulated in one launch;
+ * a feature whose plane is in the state, with use_plane_constraint and use_refine_plane_feat set and _features_SLAM_to_PLANE[featid] absent
+ * or non-zero, is a refinement candidate: every candidate is refined onto its plane (plane fixed at its current value, sigma_pix / fx of
+ * the current intrinsics) in one launch, whether or not its triangulation succeeded (the reference refines first, :147-193).  A successful
+ * refinement sets _features_SLAM_to_PLANE[featid] to the plane id; a failed one sets it to 0 when the triangulation succeeded (:195-200).
+ * Then, per triangulated feature in input order, the initialisation of ovp_slam_delayed_init: with the plane from the refined position,
+ * or without it from the triangulated position when the refinement failed; after a chi2 rejection with the plane, once more without it
+ * from the triangulated position.  The measurements cross to the device once and the Jacobians read them there; statuses and positions
+ * come back once before the initialisations.
+ * feat_status[F]: -1 fewer than 2 measurements, -2 triangulation failed, 0 not initialised, 1 initialised (with its plane constraint when it
+ * had one), 3 initialised after its plane was dropped for chi2.  plane_status[F] (may be NULL): -1 not a refinement candidate, 1 refined
+ * onto its plane, 0 refinement failed.  p_FinG_out[3F]: what the reference leaves in Feature::p_FinG (the refined position for a refined
+ * feature, also for status 3, whose landmark holds the triangulated one; zero for -1).  new_handles[F]: the landmark's handle, or -1.
+ * Only GLOBAL_3D landmarks are created.
+ * Refused before anything is copied or launched, with the state untouched: a null pointer, meas_offset not starting at 0 or decreasing, a
+ * duplicate featid, a featid that already has a landmark (OVP_ERR_ALREADY_IN_STATE), a featid below max_aruco_features (ArUco's own
+ * updater options are not taken), a measurement whose handle is not a clone or a clone observed twice, a chi2 table too short for the
+ * rows of a feature (3 per measurement with a plane, 2 without), sigma_pix <= 0, and OVP_ERR_CAPACITY for a track longer than
+ * OVP_SLAM_INIT_MAX_TRACK (64).  The state and row capacities of an initialisation depend on which features pass and are checked per
+ * feature as in ovp_slam_delayed_init: such a refusal comes after the launches and keeps the landmarks initialised before it. */
+int ovp_slam_delayed_init_tracks(ovp_ctx *ctx, const ovp_feature_tracks *t, const ovp_slam_init_options *opt, int *feat_status, int *plane_status,
+                                 double *p_FinG_out, int *new_handles);
+
 /* ---- UpdaterZeroVelocity (update/UpdaterZeroVelocity.cpp:68-318) ------------------------------------------------------- */
 typedef struct ovp_zupt_options {
   double gravity_mag;           /* VioManagerOptions.h:206 */

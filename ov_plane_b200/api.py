@@ -74,6 +74,11 @@ class PlaneInitOptions(C.Structure):
                 ("shuffle_kind", C.c_int), ("tri", C.c_void_p)]
 
 
+class SlamInitOptions(C.Structure):
+    _fields_ = [("sigma_pix", C.c_double), ("chi2_multipler", C.c_double), ("use_plane_constraint", C.c_int), ("use_refine_plane_feat", C.c_int),
+                ("tri", C.c_void_p)]
+
+
 DEBUG_LIB_PATH = os.path.join(_HERE, "lib", "libovp_debug.so")  # product sources + include/ovp_debug.h hooks (tools/, kernel unit tests)
 
 
@@ -450,6 +455,26 @@ class Context(object):
         self._ck(self.lib.ovp_plane_init_tracks(self.h, C.byref(t), C.byref(o), _p(fs), _p(pf), C.byref(npl), _p(pids), _p(ps), _p(nh), _p(cp)))
         k = npl.value
         return dict(feat_status=fs[:F], p_FinG=pf[:F], plane_ids=pids[:k], plane_status=ps[:k], new_handles=nh[:k], cp=cp[:k])
+
+    def slam_delayed_init_tracks(self, tracks, sigma_pix=1.0, chi2_mult=1.0, use_plane_constraint=True, use_refine_plane_feat=True,
+                                 tri_options=None):
+        """UpdaterSLAM::delayed_init end to end on raw tracks (the dict of plane_init_tracks; see include/ovp.h
+        ovp_slam_delayed_init_tracks).  use_plane_constraint: StateOptions::use_plane_constraint && use_plane_constraint_slamd.  Returns
+        feat_status, plane_status, p_FinG, new_handles."""
+        mo, mc = _i32(tracks["meas_offset"]), _i32(tracks["meas_clone"])
+        uv = np.ascontiguousarray(tracks["uv"], dtype=np.float32)
+        uvn = np.ascontiguousarray(tracks["uv_norm"], dtype=np.float32)
+        fid = np.ascontiguousarray(tracks["featid"], dtype=np.int64)
+        pid = np.ascontiguousarray(tracks["planeid"], dtype=np.int64)
+        F = len(mo) - 1
+        t = FeatureTracks(F, mo.ctypes.data, mc.ctypes.data, uv.ctypes.data, uvn.ctypes.data, fid.ctypes.data, pid.ctypes.data)
+        tri = _tri_options(tri_options)
+        o = SlamInitOptions(float(sigma_pix), float(chi2_mult), int(bool(use_plane_constraint)), int(bool(use_refine_plane_feat)),
+                            C.cast(C.pointer(tri), C.c_void_p) if tri is not None else None)
+        n = max(1, F)
+        fs, ps, pf, nh = np.zeros(n, dtype=np.int32), np.zeros(n, dtype=np.int32), np.zeros((n, 3)), np.zeros(n, dtype=np.int32)
+        self._ck(self.lib.ovp_slam_delayed_init_tracks(self.h, C.byref(t), C.byref(o), _p(fs), _p(ps), _p(pf), _p(nh)))
+        return dict(feat_status=fs[:F], plane_status=ps[:F], p_FinG=pf[:F], new_handles=nh[:F])
 
     # ---- UpdaterSLAM ----
     def slam_update(self, b, sigma_pix=1.0, chi2_mult=1.0, use_plane_constraint=True):

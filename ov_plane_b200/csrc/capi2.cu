@@ -551,10 +551,18 @@ struct FeatureJacobianStage {
   double *Hx(const Ctx *c) const { return W(c) + (size_t)rows * hfc; }
   double *res(const Ctx *c) const { return W(c) + (size_t)rows * (hfc + hxc); }
 };
+// A track that is already on the device, in the staging buffer below stage_base: the Jacobian reads its clone handles and pixels there
+// and lays its own slice out from stage_base up, so the track is neither copied again nor overwritten.
+struct DeviceTrack {
+  const int *clone;
+  const float *uv;
+  size_t stage_base;
+};
 // plane_handle >= 0: plane in the state (its values come from the device tables); otherwise cp / cp_fej (may be null: no plane).
+// dev (may be null): clone_handles / uv are also resident on the device there; clone_handles is still read on the host (checks, columns).
 static int stage_feature_jacobian(Ctx *c, int m, const int *clone_handles, const float *uv, const double *p_FinG, const double *p_FinG_fej,
                                   bool has_plane, int plane_handle, const double *cp, const double *cp_fej, double sigma_px, double sigma_c,
-                                  FeatureJacobianStage *j, int extra_hx_cols = 0) {
+                                  FeatureJacobianStage *j, int extra_hx_cols = 0, const DeviceTrack *dev = nullptr) {
   if (m > 64) // a size argument, not a track a feature kernel holds
     return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full: m=%d not in 1..64", m);
   const int off[2] = {0, m};
@@ -569,18 +577,28 @@ static int stage_feature_jacobian(Ctx *c, int m, const int *clone_handles, const
   const int hxc = ncal + 6 * m + (in_state ? 3 : 0) + extra_hx_cols; // extra: zero columns appended for an anchor clone (anchors.cu)
   const size_t w_bytes = (size_t)rows * (hfc + hxc + 1) * sizeof(double), uv_bytes = (size_t)m * 2 * sizeof(float);
   StageLayout L;
-  *j = {rows, hfc, hxc, L.take(w_bytes), L.take(uv_bytes)};
+  L.top = dev ? dev->stage_base : 0;
+  const size_t b_W = L.take(w_bytes);
+  *j = {rows, hfc, hxc, b_W, dev ? 0 : L.take(uv_bytes)};
+  if (dev && L.top > c->d_stage_bytes) // growing the buffer would drop the resident track: the caller reserves this slice
+    return fail(c, OVP_ERR_CAPACITY, "feature_jacobian_full: %zu staging bytes needed above the resident tracks, %zu reserved", L.top,
+                c->d_stage_bytes);
   if ((st = ensure_stage(c, L)))
     return st;
   OVP_CUDA(cudaMemsetAsync(j->W(c), 0, w_bytes, c->stream));
   JacArgs a;
   a.m = m;
-  int *dcl = c->dcols + (size_t)4 * c->Rcap;
-  float *duv = (float *)(c->d_stage + j->b_uv);
-  if ((st = stage_copy_in(c, dcl, clone_handles, m * sizeof(int))) || (st = stage_copy_in(c, duv, uv, uv_bytes)))
-    return st;
-  a.clone_handles = dcl;
-  a.uv = duv;
+  if (dev) {
+    a.clone_handles = dev->clone;
+    a.uv = dev->uv;
+  } else {
+    int *dcl = c->dcols + (size_t)4 * c->Rcap;
+    float *duv = (float *)(c->d_stage + j->b_uv);
+    if ((st = stage_copy_in(c, dcl, clone_handles, m * sizeof(int))) || (st = stage_copy_in(c, duv, uv, uv_bytes)))
+      return st;
+    a.clone_handles = dcl;
+    a.uv = duv;
+  }
   for (int i = 0; i < 3; i++) {
     a.pf[i] = p_FinG[i];
     a.pf_fej[i] = p_FinG_fej[i];
@@ -1643,11 +1661,20 @@ namespace ovp {
 int slam_update_impl(Ctx *c, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
                      const int64_t *planeid, const ovp_updater_options *opt, int use_plane, int *feat_status, double *feat_chi2);
 
+// The tracks of slam_delayed_init_core already on the device (ovp_slam_delayed_init_tracks): feature f's clone handles and pixels start at
+// measurement at[f] of clone / uv, and the staging buffer holds them below stage_base.
+struct DeviceTracks {
+  const int *clone;
+  const float *uv;
+  const int *at;
+  size_t stage_base;
+};
 // UpdaterSLAM::delayed_init, estimator half (UpdaterSLAM.cpp:225-372): per feature, in order, get_feature_jacobian_full with the
 // plane constraint when the plane is in the state, StateHelper::initialize(landmark, ..., chi2_multipler); when that fails WITH a
-// plane, detach the landmark from the plane and retry from the pre-refinement position (:310-359).
-static int slam_delayed_init_impl(Ctx *c, int F, const int *meas_offset, const int *meas_clone, const float *uv, const double *p_FinG,
-                                  const double *p_FinG_original, const int64_t *featid, const int64_t *planeid,
+// plane, detach the landmark from the plane and retry from the pre-refinement position (:310-359).  Shared by ovp_slam_delayed_init
+// (dev == nullptr: each attempt stages its track from meas_clone / uv) and ovp_slam_delayed_init_tracks (uv unused).
+static int slam_delayed_init_core(Ctx *c, int F, const int *meas_offset, const int *meas_clone, const float *uv, const DeviceTracks *dev,
+                                  const double *p_FinG, const double *p_FinG_original, const int64_t *featid, const int64_t *planeid,
                                   const ovp_updater_options *opt, int use_plane, int *feat_status, int *new_handles) {
   for (int f = 0; f < F; f++) {
     feat_status[f] = 0;
@@ -1659,10 +1686,13 @@ static int slam_delayed_init_impl(Ctx *c, int F, const int *meas_offset, const i
     if (c->slam.count(featid[f]))
       return fail(c, OVP_ERR_ALREADY_IN_STATE, "delayed_init: feature %lld already has a landmark", (long long)featid[f]);
     const int ph = slam_plane_of(c, featid[f], planeid ? planeid[f] : 0, use_plane);
+    DeviceTrack dt{};
+    if (dev)
+      dt = {dev->clone + dev->at[f], dev->uv + 2 * (size_t)dev->at[f], dev->stage_base};
     auto attempt = [&](const double *pf, int plane_h, int *acc, int *nh) -> int {
       FeatureJacobianStage j;
-      int st = stage_feature_jacobian(c, m, cl, uv + 2 * (size_t)meas_offset[f], pf, pf, plane_h >= 0, plane_h, nullptr, nullptr,
-                                      opt->sigma_pix, c->opt.sigma_constraint, &j);
+      int st = stage_feature_jacobian(c, m, cl, dev ? nullptr : uv + 2 * (size_t)meas_offset[f], pf, pf, plane_h >= 0, plane_h, nullptr, nullptr,
+                                      opt->sigma_pix, c->opt.sigma_constraint, &j, 0, dev ? &dt : nullptr);
       if (st)
         return st;
       std::vector<int> xo;
@@ -1726,7 +1756,7 @@ int ovp_slam_delayed_init(ovp_ctx *h, int F, const int *meas_offset, const int *
   Ctx *c = ovp::enter(h);
   if (F > 0 && (!meas_offset || !meas_clone || !uv || !featid || !opt || !p_FinG || !feat_status || !new_handles))
     return fail(c, OVP_ERR_BAD_ARGS, "slam_delayed_init: null argument");
-  return slam_delayed_init_impl(c, F, meas_offset, meas_clone, uv, p_FinG, p_FinG_original, featid, planeid, opt, use_plane_constraint,
+  return slam_delayed_init_core(c, F, meas_offset, meas_clone, uv, nullptr, p_FinG, p_FinG_original, featid, planeid, opt, use_plane_constraint,
                                 feat_status, new_handles);
 }
 int ovp_slam_handle(ovp_ctx *h, int64_t featid) {

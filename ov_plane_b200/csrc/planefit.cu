@@ -1348,3 +1348,4 @@ int ovp_optimize_plane(ovp_ctx *h, int n_planes, const int *feat_offset, const i
 } // extern "C"
 
 #include "plane_init_tracks.inc" // UpdaterPlane::init_vio_plane end to end on the stages above
+#include "slam_init_tracks.inc" // UpdaterSLAM::delayed_init end to end on the stages above

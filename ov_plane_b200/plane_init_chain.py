@@ -237,7 +237,7 @@ def true_plane_cp(pid):
 
 
 def tracks_scene(name="small_planes", seed=0, px_noise=0.5, keep_in_state=(), off_plane=(), inconsistent=(), noisy=(), ransac_fail_plane=0, n_single=0,
-                 n_far=0, **override):
+                 n_far=0, far_features=(), **override):
     """Scenario + raw tracks for plane initialisation.  Planes not in keep_in_state are taken out of the state.  off_plane = ((plane id, metres), ...):
     those planes' points are displaced along their normal by +-metres (RANSAC still fits them; the refinement or the initialisation's chi2
     rejects them, depending on the distance).  noisy = ((plane id, pixels), ...):
@@ -245,7 +245,7 @@ def tracks_scene(name="small_planes", seed=0, px_noise=0.5, keep_in_state=(), of
     while RANSAC and the refinement still accept it).  inconsistent:
     planes whose pixels are the scenario's own (taken through the TRUE poses while the state holds perturbed ones).  ransac_fail_plane != 0:
     six off-plane features are assigned to that (new) plane id.  n_single one-measurement candidate tracks, n_far candidates placed 100 m out
-    (the triangulation's depth check rejects them).  Returns (S, make_tracks) where make_tracks(clone_handles) gives the track dict."""
+    (the triangulation's depth check rejects them), and so are the features listed in far_features.  Returns (S, make_tracks) where make_tracks(clone_handles) gives the track dict."""
     S = synth.make_scenario(name, seed=seed, **override)
     rng = np.random.RandomState(4242 + seed)
     drop = [pl for pl in S.planes if pl[0] not in keep_in_state]
@@ -265,7 +265,7 @@ def tracks_scene(name="small_planes", seed=0, px_noise=0.5, keep_in_state=(), of
     if ransac_fail_plane:
         planeid[np.nonzero(planeid == 0)[0][:6]] = ransac_fail_plane
     cand = [f for f in range(S.F) if planeid[f] and planeid[f] not in keep_in_state and planeid[f] not in inconsistent]
-    far = cand[:n_far]
+    far = cand[:n_far] + list(far_features)
     single = cand[n_far:n_far + n_single]
     Rc, pic = jpl.quat_2_Rot(S.calib_value[:4]), S.calib_value[4:7]
     for f in far:  # 100 m out along the ray from the first camera of its track
