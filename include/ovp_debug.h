@@ -78,6 +78,15 @@ int ovp_debug_msckf_gram_landmarks(ovp_ctx *ctx, const ovp_feature_batch *b, con
 int ovp_debug_slam_update(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
                           const int64_t *planeid, const ovp_updater_options *opt, int use_plane_constraint, int *feat_status, double *feat_chi2,
                           double *raw_out);
+/* ovp_slam_update up to its Gram matrix G = [H r]^T [H r] of the stacked rows (tests/test_gpu_slam_reference.py); nothing after it runs, so
+ * the state and its bookkeeping (should_marg, the landmark-to-plane map) are left as they were.  G_out (gcap x gcap doubles) receives G
+ * column-major with leading dimension nc1 = nc + 1 (the residual last); info: [0] nc1, [1] the stacked rows the update laid out (its row
+ * offsets: 3m per landmark on its plane, 2m otherwise, whatever its status); cols_out (gcap): the state index
+ * of every compact column; feat_status / feat_chi2 (F): the per-landmark statuses and chi2; raw_out (NULL, or 72 doubles per measurement):
+ * the raw rows, as ovp_debug_slam_update returns them. */
+int ovp_debug_slam_gram(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
+                        const int64_t *planeid, const ovp_updater_options *opt, int use_plane_constraint, int gcap, double *G_out, int *info,
+                        int *cols_out, int *feat_status, double *feat_chi2, double *raw_out);
 
 #ifdef __cplusplus
 }

@@ -1936,14 +1936,16 @@ struct UpdaterSLAM {
         chi2_check = chi2tab.at(res.rows());
         st = 3;
         if (chi2 > opt.chi2_multipler * chi2_check) {
-          landmark->should_marg = true;
+          if ((int)feat.featid >= state->_options.max_aruco_features) // ArUco tags are not flagged (:600-605)
+            landmark->should_marg = true;
           status[fi] = 0;
           if (chi2_out)
             (*chi2_out)[fi] = chi2;
           continue;
         }
       } else if (chi2 > opt.chi2_multipler * chi2_check) {
-        landmark->should_marg = true;
+        if ((int)feat.featid >= state->_options.max_aruco_features) // ArUco tags are not flagged (:613-618)
+          landmark->should_marg = true;
         status[fi] = 0;
         if (chi2_out)
           (*chi2_out)[fi] = chi2;

@@ -3,7 +3,8 @@
 // tests/test_gpu_cholfused.py and tests/test_gpu_gemm.py (unit tests of chol_fused_kernel and the DMMA GEMM against NumPy), by
 // tests/test_gpu_numerics.py (the block-sparse feature path against the dense stack on the same batch) and by tests/test_gpu_compression.py
 // (the compressed update's Gram matrix, zero-pivot rule and innovation gate against long-double references) and by
-// tests/test_gpu_feature_gate.py (the per-feature chi2 gates of the MSCKF point and SLAM feature kernels).
+// tests/test_gpu_feature_gate.py (the per-feature chi2 gates of the MSCKF point and SLAM feature kernels) and by
+// tests/test_gpu_slam_reference.py (the SLAM update's Gram matrix against long double).
 #include "ovp_internal.h"
 using namespace ovp;
 
@@ -380,6 +381,49 @@ extern "C" int ovp_debug_slam_update(ovp_ctx *h, int F, const int *meas_offset, 
     if (st || !raw_out)
       return st;
     OVP_CUDA(cudaMemcpyAsync(raw_out, draw, nraw * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaStreamSynchronize(c->stream));
+    return OVP_OK;
+  };
+  st = run();
+  if (draw)
+    cudaFree(draw);
+  return st;
+}
+
+// Test hook (tests/test_gpu_slam_reference.py): ovp_slam_update up to its Gram matrix, with the state and the bookkeeping left as they were
+// (declared in include/ovp_debug.h).  Not part of the ABI in include/ovp.h.
+extern "C" int ovp_debug_slam_gram(ovp_ctx *h, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
+                                   const int64_t *planeid, const ovp_updater_options *opt, int use_plane_constraint, int gcap, double *G_out,
+                                   int *info, int *cols_out, int *feat_status, double *feat_chi2, double *raw_out) {
+  Ctx *c = ovp::enter(h);
+  if (F <= 0 || !meas_offset || !meas_clone || !uv || !featid || !opt || !G_out || !info || !cols_out || !feat_status || !feat_chi2)
+    return fail(c, OVP_ERR_BAD_ARGS, "debug_slam_gram: empty batch or null argument");
+  const size_t nraw = (size_t)3 * OVP_RAW_ROW * std::max(meas_offset[F], 1);
+  double *draw = nullptr;
+  if (raw_out) {
+    OVP_CUDA(cudaMalloc(&draw, nraw * sizeof(double)));
+    OVP_CUDA(cudaMemsetAsync(draw, 0, nraw * sizeof(double), c->stream));
+  }
+  c->dbg_raw = draw;
+  c->dbg_gram_stop = true;
+  c->dbg_slam_cols.clear();
+  c->dbg_slam_rows = 0;
+  int st = slam_update_impl(c, F, meas_offset, meas_clone, uv, featid, planeid, opt, use_plane_constraint, feat_status, feat_chi2);
+  c->dbg_raw = nullptr;
+  c->dbg_gram_stop = false;
+  auto run = [&]() -> int {
+    if (st)
+      return st;
+    const int nc = (int)c->dbg_slam_cols.size(), nc1 = nc + 1;
+    if (nc1 > gcap)
+      return fail(c, OVP_ERR_CAPACITY, "debug_slam_gram: %d columns, room for %d", nc1, gcap);
+    info[0] = nc1;
+    info[1] = c->dbg_slam_rows;
+    std::memcpy(cols_out, c->dbg_slam_cols.data(), (size_t)nc * sizeof(int));
+    OVP_CUDA(cudaMemcpy2DAsync(G_out, (size_t)nc1 * sizeof(double), c->wsG.S, (size_t)c->wsG.cap * sizeof(double), (size_t)nc1 * sizeof(double), nc1,
+                               cudaMemcpyDeviceToHost, c->stream));
+    if (raw_out)
+      OVP_CUDA(cudaMemcpyAsync(raw_out, draw, nraw * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     OVP_CUDA(cudaStreamSynchronize(c->stream));
     return OVP_OK;
   };

@@ -297,14 +297,14 @@ int join_side_stream(Ctx *c) {
   return OVP_OK;
 }
 
-// flag &= (some feat_flag[i] == 1): one block
-__global__ void any_accepted_kernel(int *flag, const int *feat_flag, int n) {
+// flag &= (some feat_flag[i] is in the accepted set: bit s of accept_mask for status s): one block
+__global__ void any_accepted_kernel(int *flag, const int *feat_flag, int n, unsigned accept_mask) {
   __shared__ int any;
   if (threadIdx.x == 0)
     any = 0;
   __syncthreads();
   for (int i = threadIdx.x; i < n; i += blockDim.x)
-    if (feat_flag[i] == 1)
+    if ((unsigned)feat_flag[i] < 32u && ((accept_mask >> feat_flag[i]) & 1u))
       any = 1;
   __syncthreads();
   if (threadIdx.x == 0 && !any)
@@ -313,7 +313,7 @@ __global__ void any_accepted_kernel(int *flag, const int *feat_flag, int n) {
 
 int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const double *d_z, const double *d_Rdiag, double gate_thresh,
                     int *d_gate_flag, double *d_chi2, bool apply, int zstride, bool defer_join, bool ht_lower, bool products_done,
-                    const int *feat_flag, int nfeat) {
+                    const int *feat_flag, int nfeat, unsigned accept_mask) {
   if (rr <= 0 || nc <= 0)
     return OVP_OK;
   {
@@ -358,7 +358,7 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
   if (!apply)
     return OVP_OK;
   if (feat_flag) {
-    any_accepted_kernel<<<1, 256, 0, c->stream>>>(flag, feat_flag, nfeat);
+    any_accepted_kernel<<<1, 256, 0, c->stream>>>(flag, feat_flag, nfeat, accept_mask);
     c->launches++;
   }
   // 6. P -= Y Y^T (lower tiles, mirrored) and the negative-diagonal check (StateHelper.cpp:176-187)  [skipped on the device when the gate
@@ -398,7 +398,7 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
 }
 
 int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, double gate_thresh, int *d_gate_flag, double *d_chi2,
-                       bool defer_join, const int *feat_flag, int nfeat) {
+                       bool defer_join, const int *feat_flag, int nfeat, unsigned accept_mask) {
   const int nc1 = nc + 1;
   const MatView L = mv(c->wsG.S, c->wsG.cap);
   const double *z = c->wsG.S + nc; // row nc of the factor, read in place (stride wsG.cap)
@@ -419,7 +419,7 @@ int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, 
       return st;
   }
   return ekf_update_core(c, d_cols, nc, L, npiv, z, nullptr, gate_thresh, d_gate_flag, d_chi2, true, c->wsG.cap, defer_join, true, fused,
-                         feat_flag, nfeat);
+                         feat_flag, nfeat, accept_mask);
 }
 
 } // namespace ovp

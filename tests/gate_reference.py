@@ -139,7 +139,7 @@ SLAM_LENGTHS = (1, 2, 15, 29)
 def slam_scenario(ncal, seed=0, F=24):
     """Landmarks tracked over 29-30 of 30 clones, half of them on one of 4 in-state planes."""
     from ov_plane_b200 import synth
-    cal = {0: (0, 0), 14: (1, 1)}[ncal]
+    cal = {0: (0, 0), 6: (1, 0), 8: (0, 1), 14: (1, 1)}[ncal]
     return synth.make_scenario("small_planes", seed=seed, n_clones=30, F=F, m_min=29, m_max=30, dtheta=0.01, calib_pose=cal[0],
                                calib_intr=cal[1])
 
