@@ -155,7 +155,14 @@ int ovp_plane_measurement_compress_inplace(ovp_ctx *ctx, double *H_x, int cols, 
                                            int *rows_out);
 
 /* ---- UpdaterMSCKF::update from "features triangulated, plane CPs known" on (UpdaterMSCKF.cpp:407-828) --------------- */
-/* Track length: every feature of a batch has 2..39 measurements, or 2..37 when the batch runs a plane update (an in-state plane,
+/* Feature tracks, as every entry point that takes them reads them (this batch, ovp_slam_update, ovp_slam_delayed_init, ovp_feature_tracks,
+ * ovp_triangulate_features, ovp_optimize_plane): meas_offset holds F + 1 prefix offsets that start at 0 and never decrease, so feature f's
+ * measurements are meas_offset[f] .. meas_offset[f + 1] - 1 of the meas_offset[F] in the measurement arrays; each measurement's handle is a
+ * clone in the state (a live pose other than the camera extrinsics); and, mono camera, a track observes each clone at most once (the
+ * triangulation and the refinement take a clone twice).  The arrays an entry point reads are non-null when F > 0 (the measurement arrays
+ * when there are measurements).  A batch that breaks this is refused with OVP_ERR_BAD_ARGS before any of it is copied or launched, with
+ * the state untouched; each entry point below states its own track-length limits.
+ * Track length: every feature of a batch has 2..39 measurements, or 2..37 when the batch runs a plane update (an in-state plane,
  * a plane not in the state with >= 4 features, or ovp_plane_init).  Tracks of up to 32 run on the block-sparse feature kernel; one
  * longer track puts the whole batch on the dense stacked one, whose per-feature system must fit the CTA's shared memory.  A longer track
  * is refused with OVP_ERR_CAPACITY before anything is launched, and the message names the limit.  Every other capacity check
@@ -163,7 +170,7 @@ int ovp_plane_measurement_compress_inplace(ovp_ctx *ctx, double *H_x, int cols, 
  * it was. */
 typedef struct ovp_feature_batch {
   int F;                         /* number of features (feature_vec after triangulation, caller's order)               */
-  const int *meas_offset;        /* F+1 prefix offsets into the measurement arrays                                      */
+  const int *meas_offset;        /* F+1 prefix offsets into the measurement arrays (feature tracks, above)             */
   const int *meas_clone;         /* per measurement: handle of the clone it was taken at (Feature::timestamps)          */
   const float *uv;               /* per measurement: raw pixel (u,v) as float, like Feature::uvs (Eigen::VectorXf)       */
   const double *p_FinG;          /* 3F: triangulated (and, for on-plane features, plane-refined) position               */
@@ -224,7 +231,11 @@ int ovp_slam_update(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas
                     double *feat_chi2);
 /* UpdaterSLAM::delayed_init from "8. Finally, initialize" on (:225-372): per feature, in order, Jacobians at p_FinG (FEJ =
  * value), StateHelper::initialize(Landmark, ..., chi2_multipler); a failure WITH a plane retries without it from
- * p_FinG_original (:310-359).  feat_status[f]: 1 / 3 as above, 0 not initialised; new_handles[f]: landmark handle or -1. */
+ * p_FinG_original (:310-359).  feat_status[f]: 1 / 3 as above, 0 not initialised; new_handles[f]: landmark handle or -1.
+ * Every track has 1..64 measurements, from clones with or without covariance columns; every track is checked before the first landmark is
+ * initialised, and a malformed one is refused with OVP_ERR_BAD_ARGS with the state untouched.  A featid that already has a landmark
+ * (OVP_ERR_ALREADY_IN_STATE), a clone without covariance columns (OVP_ERR_NOT_IN_STATE) and the state's capacity are checked per feature,
+ * in order: such a refusal keeps the landmarks initialised before it. */
 int ovp_slam_delayed_init(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv, const double *p_FinG,
                           const double *p_FinG_original, const int64_t *featid, const int64_t *planeid,
                           const ovp_updater_options *opt, int use_plane_constraint, int *feat_status, int *new_handles);
@@ -299,14 +310,15 @@ typedef struct ovp_triangulation_options {
  * that live in the context: meas_offset / meas_clone as in ovp_feature_batch (measurements in time order: the anchor is the last
  * one), uv_norm = Feature::uvs_norm (undistorted normalised coordinates, 2 floats per measurement).  status[f] = 1: p_FinG[3f..]
  * is the refined position; 0: the reference would drop the feature (condition number, depth range, baseline ratio, NaN).
- * opt == NULL runs the defaults.  Refused with OVP_ERR_BAD_ARGS before anything is copied or launched: a null pointer, meas_offset not
- * starting at 0 or decreasing (so no track reaches past meas_offset[F]), a measurement whose handle is not a clone. */
+ * opt == NULL runs the defaults.  Tracks of any length, a clone observed twice included; malformed tracks and a null pointer are refused
+ * with OVP_ERR_BAD_ARGS before anything is copied or launched. */
 int ovp_triangulate_features(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv_norm,
                              const ovp_triangulation_options *opt, double *p_FinG, int *status);
 
 /* ---- PlaneFitting (track_plane/PlaneFitting.cpp): plane hypothesis + refinement, the step right before the plane Jacobians ----------- */
 /* Call sites: UpdaterMSCKF.cpp:267-360, UpdaterPlane.cpp:230-267, UpdaterSLAM.cpp:171.  Both entry points take a BATCH of candidate planes
- * (feat_offset: n_planes + 1 prefix offsets into the per-feature arrays) and run them concurrently. */
+ * (feat_offset: n_planes + 1 prefix offsets into the per-feature arrays, starting at 0 and never decreasing, else OVP_ERR_BAD_ARGS) and run
+ * them concurrently. */
 typedef struct ovp_plane_fit_options {
   int min_inlier_num;     /* StateOptions::plane_msckf_min_feat / plane_init_min_feat */
   double max_cond_number; /* StateOptions::plane_msckf_max_cond / plane_init_max_cond */
@@ -371,8 +383,8 @@ typedef struct ovp_plane_init_options {
  * with a candidate after triangulation, ascending id; plane_status 1 initialised, 0 rejected by initialize's chi2, -2 RANSAC returned false,
  * -3 optimize_plane returned false, -1 not attempted (fewer than 3 features left); new_handles (or -1); cp_out[3 * n_planes] the
  * linearisation point handed to initialize (the refinement's plane, zero when RANSAC failed).
- * Refused before anything is copied or launched, with the state untouched: a null pointer, meas_offset not starting at 0 or decreasing, a
- * duplicate featid, a candidate measurement whose handle is not a clone (or that observes a clone twice), OVP_ERR_CAPACITY for a candidate
+ * Refused before anything is copied or launched, with the state untouched: a null pointer, malformed tracks (a candidate's per-track rules
+ * only), a duplicate featid, OVP_ERR_CAPACITY for a candidate
  * track longer than the plane-system limit (37, see ovp_msckf_update) or max_msckf_plane + 1 above RANSAC's 1900 points.  The capacities of
  * the initialisation stage itself (rows of one plane's stacked system against max_meas_rows, three more state rows per new plane against
  * max_state) depend on RANSAC's and the refinement's outcome and are checked by that stage as in ovp_plane_init: such a refusal comes after
@@ -405,9 +417,9 @@ typedef struct ovp_slam_init_options {
  * onto its plane, 0 refinement failed.  p_FinG_out[3F]: what the reference leaves in Feature::p_FinG (the refined position for a refined
  * feature, also for status 3, whose landmark holds the triangulated one; zero for -1).  new_handles[F]: the landmark's handle, or -1.
  * Only GLOBAL_3D landmarks are created.
- * Refused before anything is copied or launched, with the state untouched: a null pointer, meas_offset not starting at 0 or decreasing, a
- * duplicate featid, a featid that already has a landmark (OVP_ERR_ALREADY_IN_STATE), a featid below max_aruco_features (ArUco's own
- * updater options are not taken), a measurement whose handle is not a clone or a clone observed twice, a chi2 table too short for the
+ * Refused before anything is copied or launched, with the state untouched: a null pointer, malformed tracks (the per-track rules for the
+ * tracks of two or more measurements), a duplicate featid, a featid that already has a landmark (OVP_ERR_ALREADY_IN_STATE), a featid below
+ * max_aruco_features (ArUco's own updater options are not taken), a chi2 table too short for the
  * rows of a feature (3 per measurement with a plane, 2 without), sigma_pix <= 0, and OVP_ERR_CAPACITY for a track longer than
  * OVP_SLAM_INIT_MAX_TRACK (64).  The state and row capacities of an initialisation depend on which features pass and are checked per
  * feature as in ovp_slam_delayed_init: such a refusal comes after the launches and keeps the landmarks initialised before it. */

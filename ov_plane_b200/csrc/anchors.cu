@@ -110,8 +110,8 @@ int ovp_feature_jacobian_full_rep(ovp_ctx *h, int m, const int *clone_handles, c
   const bool rel = is_relative(representation);
   if (rel && !is_clone(c, anchor_clone_handle, true))
     return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full_rep: anchor handle %d is not a clone in the state", anchor_clone_handle);
-  int st = sync_host_values(c);
-  if (st)
+  int st = check_jacobian_track(c, "feature_jacobian_full_rep", m, clone_handles);
+  if (st || (st = sync_host_values(c)))
     return st;
   double pG[3] = {p_F[0], p_F[1], p_F[2]}, pGf[3] = {p_F_fej[0], p_F_fej[1], p_F_fej[2]};
   const double *cal = c->h_val.data() + (size_t)c->h_calib * OVP_VAL_STRIDE;

@@ -432,8 +432,8 @@ extern "C" {
 
 int ovp_plane_init(ovp_ctx *h, const ovp_feature_batch *batch, const ovp_updater_options *opt, int *plane_status, int *new_handles) {
   Ctx *c = ovp::enter(h);
-  if (!batch || !opt || !batch->plane_cp)
-    return fail(c, OVP_ERR_BAD_ARGS, "plane_init: null batch / options / plane_cp");
+  if (!batch || !opt || !batch->plane_cp || (batch->F > 0 && !batch->planeid))
+    return fail(c, OVP_ERR_BAD_ARGS, "plane_init: null batch / options / plane_cp / planeid");
   return ovp::plane_init_core(c, batch, opt, plane_status, new_handles);
 }
 
@@ -558,18 +558,19 @@ struct DeviceTrack {
   const float *uv;
   size_t stage_base;
 };
+// The one track of get_feature_jacobian_full: 1..64 measurements (a size argument, not a track a feature kernel holds, so a longer one is a
+// bad argument), each from a live pose with or without covariance columns, observed once.
+static int check_jacobian_track(Ctx *c, const char *who, int m, const int *clone_handles) {
+  const int off[2] = {0, m};
+  return check_tracks(c, who, 1, off, clone_handles, nullptr, 1, 64, OVP_ERR_BAD_ARGS, false, true);
+}
 // plane_handle >= 0: plane in the state (its values come from the device tables); otherwise cp / cp_fej (may be null: no plane).
-// dev (may be null): clone_handles / uv are also resident on the device there; clone_handles is still read on the host (checks, columns).
+// dev (may be null): clone_handles / uv are also resident on the device there; clone_handles is still read on the host (columns).  The
+// caller has checked the track (check_jacobian_track or its own check_tracks).
 static int stage_feature_jacobian(Ctx *c, int m, const int *clone_handles, const float *uv, const double *p_FinG, const double *p_FinG_fej,
                                   bool has_plane, int plane_handle, const double *cp, const double *cp_fej, double sigma_px, double sigma_c,
                                   FeatureJacobianStage *j, int extra_hx_cols = 0, const DeviceTrack *dev = nullptr) {
-  if (m > 64) // a size argument, not a track a feature kernel holds
-    return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full: m=%d not in 1..64", m);
-  const int off[2] = {0, m};
-  int mmax;
-  int st = check_tracks(c, 1, off, clone_handles, 1, 0, false, &mmax); // a live pose, with or without covariance columns
-  if (st)
-    return st;
+  int st;
   const bool in_state = has_plane && plane_handle >= 0;
   const int ncal = (c->opt.do_calib_camera_pose ? 6 : 0) + (c->opt.do_calib_camera_intrinsics ? 8 : 0);
   const int rows = has_plane ? 3 * m : 2 * m;
@@ -713,11 +714,14 @@ int ovp_feature_jacobian_full(ovp_ctx *h, int m, const int *clone_handles, const
                               int64_t planeid, const double *cp, const double *cp_fej, double sigma_px, double sigma_c, double *H_f,
                               int *hf_cols, double *H_x, int *hx_cols, double *res, int *rows_out, int *x_order, int *x_order_n) {
   Ctx *c = ovp::enter(h);
+  int st = check_jacobian_track(c, "feature_jacobian_full", m, clone_handles);
+  if (st)
+    return st;
   const bool has_plane = planeid != 0;
   const bool in_state = has_plane && c->planes.count(planeid);
   FeatureJacobianStage j;
-  int st = stage_feature_jacobian(c, m, clone_handles, uv, p_FinG, p_FinG_fej, has_plane, in_state ? c->planes[planeid] : -1, cp, cp_fej,
-                                  sigma_px, sigma_c, &j);
+  st = stage_feature_jacobian(c, m, clone_handles, uv, p_FinG, p_FinG_fej, has_plane, in_state ? c->planes[planeid] : -1, cp, cp_fej,
+                              sigma_px, sigma_c, &j);
   if (st || (st = read_feature_jacobian(c, j, j.hfc, H_f, H_x, res)))
     return st;
   *hf_cols = j.hfc;
@@ -1756,6 +1760,10 @@ int ovp_slam_delayed_init(ovp_ctx *h, int F, const int *meas_offset, const int *
   Ctx *c = ovp::enter(h);
   if (F > 0 && (!meas_offset || !meas_clone || !uv || !featid || !opt || !p_FinG || !feat_status || !new_handles))
     return fail(c, OVP_ERR_BAD_ARGS, "slam_delayed_init: null argument");
+  // every track is checked before the first landmark is initialised (each one's Jacobian takes 1..64 measurements)
+  int st = check_tracks(c, "slam_delayed_init", F, meas_offset, meas_clone, nullptr, 1, 64, OVP_ERR_BAD_ARGS, false, true);
+  if (st)
+    return st;
   return slam_delayed_init_core(c, F, meas_offset, meas_clone, uv, nullptr, p_FinG, p_FinG_original, featid, planeid, opt, use_plane_constraint,
                                 feat_status, new_handles);
 }

@@ -368,14 +368,18 @@ extern "C" int ovp_debug_slam_update(ovp_ctx *h, int F, const int *meas_offset, 
   Ctx *c = ovp::enter(h);
   if (F > 0 && (!meas_offset || !meas_clone || !uv || !featid || !opt))
     return fail(c, OVP_ERR_BAD_ARGS, "debug_slam_update: null argument");
-  const size_t nraw = (size_t)3 * OVP_RAW_ROW * std::max(F > 0 ? meas_offset[F] : 0, 1);
+  int M = 0;
+  int st = check_offsets(c, "debug_slam_update", "meas_offset", F, meas_offset, &M);
+  if (st)
+    return st;
+  const size_t nraw = (size_t)3 * OVP_RAW_ROW * std::max(M, 1);
   double *draw = nullptr;
   if (raw_out) {
     OVP_CUDA(cudaMalloc(&draw, nraw * sizeof(double)));
     OVP_CUDA(cudaMemsetAsync(draw, 0, nraw * sizeof(double), c->stream));
   }
   c->dbg_raw = draw;
-  int st = slam_update_impl(c, F, meas_offset, meas_clone, uv, featid, planeid, opt, use_plane_constraint, feat_status, feat_chi2);
+  st = slam_update_impl(c, F, meas_offset, meas_clone, uv, featid, planeid, opt, use_plane_constraint, feat_status, feat_chi2);
   c->dbg_raw = nullptr;
   auto run = [&]() -> int {
     if (st || !raw_out)
@@ -398,7 +402,11 @@ extern "C" int ovp_debug_slam_gram(ovp_ctx *h, int F, const int *meas_offset, co
   Ctx *c = ovp::enter(h);
   if (F <= 0 || !meas_offset || !meas_clone || !uv || !featid || !opt || !G_out || !info || !cols_out || !feat_status || !feat_chi2)
     return fail(c, OVP_ERR_BAD_ARGS, "debug_slam_gram: empty batch or null argument");
-  const size_t nraw = (size_t)3 * OVP_RAW_ROW * std::max(meas_offset[F], 1);
+  int M = 0;
+  int st = check_offsets(c, "debug_slam_gram", "meas_offset", F, meas_offset, &M);
+  if (st)
+    return st;
+  const size_t nraw = (size_t)3 * OVP_RAW_ROW * std::max(M, 1);
   double *draw = nullptr;
   if (raw_out) {
     OVP_CUDA(cudaMalloc(&draw, nraw * sizeof(double)));
@@ -408,7 +416,7 @@ extern "C" int ovp_debug_slam_gram(ovp_ctx *h, int F, const int *meas_offset, co
   c->dbg_gram_stop = true;
   c->dbg_slam_cols.clear();
   c->dbg_slam_rows = 0;
-  int st = slam_update_impl(c, F, meas_offset, meas_clone, uv, featid, planeid, opt, use_plane_constraint, feat_status, feat_chi2);
+  st = slam_update_impl(c, F, meas_offset, meas_clone, uv, featid, planeid, opt, use_plane_constraint, feat_status, feat_chi2);
   c->dbg_raw = nullptr;
   c->dbg_gram_stop = false;
   auto run = [&]() -> int {

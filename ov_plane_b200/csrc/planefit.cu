@@ -1165,28 +1165,19 @@ int ovp_triangulate_features(ovp_ctx *h, int F, const int *meas_offset, const in
     return OVP_OK;
   if (!meas_offset || !meas_clone || !uv_norm || !p_FinG || !status)
     return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: null argument");
-  // a track must not reach past the M = meas_offset[F] measurements that are staged
-  if (meas_offset[0] != 0)
-    return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: meas_offset must start at 0");
-  for (int f = 0; f < F; f++)
-    if (meas_offset[f + 1] < meas_offset[f])
-      return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: meas_offset is not non-decreasing at feature %d", f);
-  const int M = meas_offset[F];
-  for (int k = 0; k < M; k++)
-    if (!is_clone(c, meas_clone[k], true))
-      return fail(c, OVP_ERR_BAD_ARGS, "triangulate_features: measurement %d: handle %d is not a clone in the state", k, meas_clone[k]);
-  if (c->var_table_dirty) {
-    int st = upload_var_table(c);
-    if (st)
-      return st;
-  }
+  // a track of any length, but it must not reach past the M = meas_offset[F] measurements that are staged
+  int M = 0;
+  int st = check_tracks(c, "triangulate_features", F, meas_offset, meas_clone, nullptr, 0, 0, 0, true, false, &M);
+  if (st)
+    return st;
+  if (c->var_table_dirty && (st = upload_var_table(c)))
+    return st;
   // staging: [offsets | clones | uvn] in, [p_FinG | status] out, camera pose table
   StageLayout L;
   const size_t b_off = L.take((size_t)(F + 1) * 4), b_cl = L.take((size_t)M * 4), b_uv = L.take((size_t)M * 8), b_pf = L.take((size_t)F * 24),
                b_st = L.take((size_t)F * 4);
   const PoseTable pose(L, (int)c->vars.size());
-  int st = ensure_stage(c, L);
-  if (st)
+  if ((st = ensure_stage(c, L)))
     return st;
   char *d = c->d_stage;
   if ((st = stage_copy_in(c, d + b_off, meas_offset, (size_t)(F + 1) * 4)) || (st = stage_copy_in(c, d + b_cl, meas_clone, (size_t)M * 4)) ||
@@ -1224,12 +1215,13 @@ int ovp_plane_fitting(ovp_ctx *h, int n_planes, const int *feat_offset, const do
     return fail(c, OVP_ERR_BAD_ARGS, "plane_fitting: null argument");
   if (opt->shuffle_kind != 0 && opt->shuffle_kind != 1)
     return fail(c, OVP_ERR_BAD_ARGS, "plane_fitting: shuffle_kind %d (0 = libstdc++ GCC <= 10, 1 = GCC >= 11)", opt->shuffle_kind);
-  if (feat_offset[0] != 0)
-    return fail(c, OVP_ERR_BAD_ARGS, "plane_fitting: feat_offset must start at 0");
-  const int Ftot = feat_offset[n_planes];
+  int Ftot = 0;
+  int st = check_offsets(c, "plane_fitting", "feat_offset", n_planes, feat_offset, &Ftot);
+  if (st)
+    return st;
   for (int p = 0; p < n_planes; p++) {
     const int F = feat_offset[p + 1] - feat_offset[p];
-    if (F < 0 || F > PF_MAX_POINTS)
+    if (F > PF_MAX_POINTS)
       return fail(c, OVP_ERR_CAPACITY, "plane_fitting: plane %d has %d points (limit %d)", p, F, PF_MAX_POINTS);
   }
   if (Ftot == 0) {
@@ -1246,8 +1238,7 @@ int ovp_plane_fitting(ovp_ctx *h, int n_planes, const int *feat_offset, const do
   const size_t b_fo = L.take((size_t)(n_planes + 1) * 4), b_po = L.take((size_t)n_planes * 4), b_pm = L.take(plan.perms.size() * 4),
                b_pt = L.take((size_t)Ftot * 24), b_in_end = L.top;
   const RansacOut out(L, n_planes, Ftot);
-  int st = ensure_stage(c, L);
-  if (st)
+  if ((st = ensure_stage(c, L)))
     return st;
   std::vector<char> hbuf(b_in_end);
   std::memcpy(hbuf.data() + b_fo, feat_offset, (size_t)(n_planes + 1) * 4);
@@ -1274,23 +1265,15 @@ int ovp_optimize_plane(ovp_ctx *h, int n_planes, const int *feat_offset, const i
     return OVP_OK;
   if (!feat_offset || !meas_offset || !p_FinG || !cp_inG || !fix_plane || !opt || !p_FinG_out || !cp_out || !inlier || !status)
     return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: null argument");
-  if (feat_offset[0] != 0 || meas_offset[0] != 0)
-    return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: offset arrays must start at 0");
-  for (int p = 0; p < n_planes; p++)
-    if (feat_offset[p + 1] < feat_offset[p])
-      return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: feat_offset is not non-decreasing at plane %d", p);
-  const int Ftot = feat_offset[n_planes];
-  for (int f = 0; f < Ftot; f++)
-    if (meas_offset[f + 1] < meas_offset[f])
-      return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: meas_offset is not non-decreasing at feature %d", f);
-  const int M = (Ftot > 0) ? meas_offset[Ftot] : 0;
-  if (M > 0 && (!meas_clone || !uv_norm))
-    return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: null measurement arrays");
+  // the tracks of the Ftot = feat_offset[n_planes] features, of any length (a SLAM feature has none)
+  int Ftot = 0, M = 0;
+  int st = check_offsets(c, "optimize_plane", "feat_offset", n_planes, feat_offset, &Ftot);
+  if (st || (st = check_tracks(c, "optimize_plane", Ftot, meas_offset, meas_clone, nullptr, 0, 0, 0, true, false, &M)))
+    return st;
+  if (M > 0 && !uv_norm)
+    return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: null uv_norm");
   if (!(opt->sigma_px_norm > 0.0) || !(opt->sigma_c > 0.0))
     return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: sigma_px_norm / sigma_c must be positive");
-  for (int k = 0; k < M; k++)
-    if (!is_clone(c, meas_clone[k], true))
-      return fail(c, OVP_ERR_BAD_ARGS, "optimize_plane: measurement %d: handle %d is not a clone in the state", k, meas_clone[k]);
   if (Ftot == 0) {
     for (int p = 0; p < n_planes; p++) {
       status[p] = 0;
@@ -1302,13 +1285,9 @@ int ovp_optimize_plane(ovp_ctx *h, int n_planes, const int *feat_offset, const i
     }
     return OVP_OK;
   }
-  if (c->var_table_dirty) {
-    int st = upload_var_table(c);
-    if (st)
-      return st;
-  }
-  int st = sync_host_values(c); // the current IMU pose and the extrinsics of the in-front-of-camera test
-  if (st)
+  if (c->var_table_dirty && (st = upload_var_table(c)))
+    return st;
+  if ((st = sync_host_values(c))) // the current IMU pose and the extrinsics of the in-front-of-camera test
     return st;
   // staging: [feat_offset | meas_offset | meas_clone | uvn | fix | p0 | cp0] in, camera pose table, the refinement's outputs
   StageLayout L;
