@@ -60,14 +60,18 @@ void UpdaterSLAM::update(std::shared_ptr<State> state, std::vector<std::shared_p
   Flat fl;
   for (auto &f : feature_vec)
     fl.append(state, *f, feat2plane);
+  // the ArUco tags among them whiten and gate with _options_aruco (:500, :545-547); host-only, set on every call since the constructor has
+  // no state to hand them to
+  const ovp_updater_options ua = {_options_aruco.sigma_pix, _options_aruco.chi2_multipler};
+  ck(state->ctx, ovp_set_aruco_options(state->ctx, &ua));
   ovp_updater_options uo = {_options_slam.sigma_pix, _options_slam.chi2_multipler};
   std::vector<int> st(feature_vec.size());
   std::vector<double> chi(feature_vec.size());
   ck(state->ctx, ovp_slam_update(state->ctx, (int)feature_vec.size(), fl.meas_offset.data(), fl.meas_clone.data(), fl.uv.data(), fl.featid.data(),
                                  fl.planeid.data(), &uo, state->_options.use_plane_constraint_slamu ? 1 : 0, st.data(), chi.data()));
-  for (size_t i = 0; i < feature_vec.size(); i++) { // 0: rejected -> the landmark is flagged for marginalisation (:659-668)
+  for (size_t i = 0; i < feature_vec.size(); i++) { // 0: rejected -> the landmark is flagged for marginalisation unless a tag (:596-618)
     feature_vec[i]->to_delete = true;
-    if (st[i] == 0)
+    if (st[i] == 0 && (int)feature_vec[i]->featid >= state->_options.max_aruco_features)
       state->_features_SLAM.at(feature_vec[i]->featid)->should_marg = true;
     if (st[i] == 3)
       state->_features_SLAM_to_PLANE[feature_vec[i]->featid] = 0; // accepted only without its plane (:594-609)
@@ -76,16 +80,11 @@ void UpdaterSLAM::update(std::shared_ptr<State> state, std::vector<std::shared_p
 
 void UpdaterSLAM::delayed_init(std::shared_ptr<State> state, std::vector<std::shared_ptr<ov_core::Feature>> &feature_vec,
                                const std::map<size_t, size_t> &feat2plane) {
-  // ArUco features (featid < max_aruco_features) need UpdaterSLAM's separate ArUco options, which the library does not take: they are left
-  // in feature_vec as they came, not initialised (use_aruco is false in every shipped config, so none arrive there)
-  std::vector<std::shared_ptr<ov_core::Feature>> aruco, slam;
-  for (auto &f : feature_vec)
-    ((int)f->featid < state->_options.max_aruco_features ? aruco : slam).push_back(f);
-  feature_vec.swap(slam);
-  if (feature_vec.empty()) {
-    feature_vec.swap(aruco);
+  if (feature_vec.empty())
     return;
-  }
+  // ArUco features (featid < max_aruco_features) are initialised with _options_aruco (:164, :257, :302-304), in the same call as the rest
+  const ovp_updater_options ua = {_options_aruco.sigma_pix, _options_aruco.chi2_multipler};
+  ck(state->ctx, ovp_set_aruco_options(state->ctx, &ua));
   // :77-103 clean every track against the clone times
   std::vector<double> clonetimes;
   for (const auto &clone_imu : state->_clones_IMU)
@@ -114,7 +113,7 @@ void UpdaterSLAM::delayed_init(std::shared_ptr<State> state, std::vector<std::sh
   std::vector<int> feat_status(F), new_handles(F);
   std::vector<double> p_FinG(3 * F);
   ck(state->ctx, ovp_slam_delayed_init_tracks(state->ctx, &t, &o, feat_status.data(), nullptr, p_FinG.data(), new_handles.data()));
-  std::vector<std::shared_ptr<ov_core::Feature>> kept(aruco);
+  std::vector<std::shared_ptr<ov_core::Feature>> kept;
   for (size_t i = 0; i < F; i++) {
     auto &f = feature_vec[i];
     f->to_delete = true; // every feature of the call (:98, :190, :306-361)

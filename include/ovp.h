@@ -242,6 +242,13 @@ int ovp_slam_delayed_init(ovp_ctx *ctx, int F, const int *meas_offset, const int
 int ovp_slam_handle(ovp_ctx *ctx, int64_t featid);       /* State::_features_SLAM lookup; -1 = absent */
 int ovp_slam_should_marg(ovp_ctx *ctx, int64_t featid);  /* Landmark::should_marg (1/0), -1 = absent */
 int64_t ovp_slam_plane_of(ovp_ctx *ctx, int64_t featid); /* State::_features_SLAM_to_PLANE entry, -1 = no entry */
+/* UpdaterSLAM's options_aruco (UpdaterSLAM.h; UpdaterSLAM.cpp:164, 257, 302-304, 500, 545-547): once set, ovp_slam_update,
+ * ovp_slam_delayed_init and ovp_slam_delayed_init_tracks whiten and gate every feature with featid < max_aruco_features (an ArUco tag
+ * corner) with these instead of the call's own options: its bearing rows (not its point-on-plane rows, which keep sigma_constraint), its
+ * chi2 gates with and without the plane, and in ovp_slam_delayed_init_tracks its single-feature refinement (sigma_pix / fx).  NULL clears
+ * them (the default: every feature takes the call's options, and ovp_slam_delayed_init_tracks refuses ArUco ids).  sigma_pix <= 0 or
+ * chi2_multipler <= 0: OVP_ERR_BAD_ARGS, the options held before are kept.  Host-only: nothing is copied to the device. */
+int ovp_set_aruco_options(ovp_ctx *ctx, const ovp_updater_options *aruco);
 
 /* ---- Anchored landmark representations (UpdaterHelper.cpp:35-193, UpdaterSLAM.cpp:684-850) -------------------------------------------- */
 /* get_feature_jacobian_full (UpdaterHelper.cpp:195-449) for any ov_type::LandmarkRepresentation (numbering as in
@@ -419,7 +426,7 @@ typedef struct ovp_slam_init_options {
  * Only GLOBAL_3D landmarks are created.
  * Refused before anything is copied or launched, with the state untouched: a null pointer, malformed tracks (the per-track rules for the
  * tracks of two or more measurements), a duplicate featid, a featid that already has a landmark (OVP_ERR_ALREADY_IN_STATE), a featid below
- * max_aruco_features (ArUco's own updater options are not taken), a chi2 table too short for the
+ * max_aruco_features while no ArUco options are set (ovp_set_aruco_options; with them tags are accepted), a chi2 table too short for the
  * rows of a feature (3 per measurement with a plane, 2 without), sigma_pix <= 0, and OVP_ERR_CAPACITY for a track longer than
  * OVP_SLAM_INIT_MAX_TRACK (64).  The state and row capacities of an initialisation depend on which features pass and are checked per
  * feature as in ovp_slam_delayed_init: such a refusal comes after the launches and keeps the landmarks initialised before it. */

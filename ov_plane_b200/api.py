@@ -502,6 +502,16 @@ class Context(object):
                                                 int(bool(use_plane_constraint)), _p(fs), _p(nh)))
         return dict(feat_status=fs[:F], new_handles=nh[:F])
 
+    def set_aruco_options(self, sigma_pix, chi2_mult=1.0):
+        """UpdaterSLAM's options_aruco: slam_update, slam_delayed_init and slam_delayed_init_tracks whiten and gate every feature with
+        featid < max_aruco_features with these instead of the call's options (include/ovp.h ovp_set_aruco_options).  sigma_pix=None
+        clears them: every feature takes the call's options again and slam_delayed_init_tracks refuses ArUco ids."""
+        if sigma_pix is None:
+            self._ck(self.lib.ovp_set_aruco_options(self.h, None))
+            return
+        uo = UpdaterOptions(float(sigma_pix), float(chi2_mult))
+        self._ck(self.lib.ovp_set_aruco_options(self.h, C.byref(uo)))
+
     def slam_handle(self, featid):
         return self.lib.ovp_slam_handle(self.h, C.c_int64(int(featid)))
 

@@ -1675,7 +1675,8 @@ struct DeviceTracks {
 };
 // UpdaterSLAM::delayed_init, estimator half (UpdaterSLAM.cpp:225-372): per feature, in order, get_feature_jacobian_full with the
 // plane constraint when the plane is in the state, StateHelper::initialize(landmark, ..., chi2_multipler); when that fails WITH a
-// plane, detach the landmark from the plane and retry from the pre-refinement position (:310-359).  Shared by ovp_slam_delayed_init
+// plane, detach the landmark from the plane and retry from the pre-refinement position (:310-359).  An ArUco tag takes the context's
+// ArUco options on both tries (slam_options_of).  Shared by ovp_slam_delayed_init
 // (dev == nullptr: each attempt stages its track from meas_clone / uv) and ovp_slam_delayed_init_tracks (uv unused).
 static int slam_delayed_init_core(Ctx *c, int F, const int *meas_offset, const int *meas_clone, const float *uv, const DeviceTracks *dev,
                                   const double *p_FinG, const double *p_FinG_original, const int64_t *featid, const int64_t *planeid,
@@ -1693,10 +1694,11 @@ static int slam_delayed_init_core(Ctx *c, int F, const int *meas_offset, const i
     DeviceTrack dt{};
     if (dev)
       dt = {dev->clone + dev->at[f], dev->uv + 2 * (size_t)dev->at[f], dev->stage_base};
+    const ovp_updater_options &fo = slam_options_of(c, featid[f], *opt); // an ArUco tag's own (UpdaterSLAM.cpp:257, 302-304)
     auto attempt = [&](const double *pf, int plane_h, int *acc, int *nh) -> int {
       FeatureJacobianStage j;
       int st = stage_feature_jacobian(c, m, cl, dev ? nullptr : uv + 2 * (size_t)meas_offset[f], pf, pf, plane_h >= 0, plane_h, nullptr, nullptr,
-                                      opt->sigma_pix, c->opt.sigma_constraint, &j, 0, dev ? &dt : nullptr);
+                                      fo.sigma_pix, c->opt.sigma_constraint, &j, 0, dev ? &dt : nullptr);
       if (st)
         return st;
       std::vector<int> xo;
@@ -1719,7 +1721,7 @@ static int slam_delayed_init_core(Ctx *c, int F, const int *meas_offset, const i
         if (st)
           return st;
       }
-      return initialize_core(c, OVP_KIND_LANDMARK, 3, pf, pf, featid[f], c->dcols, n, j.W(c), j.rows, j.rows, j.rows, 1.0, opt->chi2_multipler,
+      return initialize_core(c, OVP_KIND_LANDMARK, 3, pf, pf, featid[f], c->dcols, n, j.W(c), j.rows, j.rows, j.rows, 1.0, fo.chi2_multipler,
                              1, acc, nh);
     };
     int acc = 0, nh = -1;
@@ -1766,6 +1768,19 @@ int ovp_slam_delayed_init(ovp_ctx *h, int F, const int *meas_offset, const int *
     return st;
   return slam_delayed_init_core(c, F, meas_offset, meas_clone, uv, nullptr, p_FinG, p_FinG_original, featid, planeid, opt, use_plane_constraint,
                                 feat_status, new_handles);
+}
+int ovp_set_aruco_options(ovp_ctx *h, const ovp_updater_options *aruco) {
+  Ctx *c = &h->c; // host-only: the kernels take the options as launch arguments
+  if (!aruco) {
+    c->has_aruco = false;
+    return OVP_OK;
+  }
+  if (!(aruco->sigma_pix > 0.0) || !(aruco->chi2_multipler > 0.0))
+    return fail(c, OVP_ERR_BAD_ARGS, "set_aruco_options: sigma_pix (%g) and chi2_multipler (%g) must be positive", aruco->sigma_pix,
+                aruco->chi2_multipler);
+  c->aruco = *aruco;
+  c->has_aruco = true;
+  return OVP_OK;
 }
 int ovp_slam_handle(ovp_ctx *h, int64_t featid) {
   auto it = h->c.slam.find(featid);

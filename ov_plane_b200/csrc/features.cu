@@ -46,6 +46,7 @@ struct FeatArgs {
   const double *plane_cp; // mode 1, plane not in the state: its 3 linearisation values in the batch staging buffer (read through
                           // the pointer so that a replayed CUDA graph sees the values of THIS call, not of the capture call)
   double white_px, white_c;
+  const double *feat_opt; // feature_kernel<true> (mode 2): per feature (global index) {white_px, chi2_mult} instead of the two below
   const double *P;
   int ldP;
   const int *state2compact;
@@ -160,7 +161,9 @@ __device__ double gate_chi2(const double *A, int lda, double *T, double *S, int 
 
 // Local column layout of the feature block A (col-major, stride lda):
 //   [0,3) H_f | [3, 3+cf) H_x = [extrinsics 6][intrinsics 8][clone_0 6]...[clone_{m-1} 6] | [3+cf, 3+cf+3) H_cp | last: res
-__global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
+// TAGS (ovp_slam_update with an ArUco tag in the batch): every feature's whitening and chi2 multiplier come from a.feat_opt.  The
+// instantiation without it is the kernel of every other launch, compiled as if the per-feature options did not exist.
+template <bool TAGS> __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
   extern __shared__ double sm[];
   const int tid = threadIdx.x;
   const int f = a.feat_sel[blockIdx.x];
@@ -217,7 +220,8 @@ __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
       pff = pf;
     }
     double res[2], Hf[6], Hcl[12], Hcal[12], Hin[16];
-    bearing_rows(vc, vc + 4, fc, fc + 4, a.do_fej, R_C, vcal + 4, cam, pf, pff, a.uv[2 * (m0 + k)], a.uv[2 * (m0 + k) + 1], a.white_px,
+    const double white_px = TAGS ? a.feat_opt[2 * f] : a.white_px; // an ArUco tag's own sigma_pix (UpdaterSLAM.cpp:500)
+    bearing_rows(vc, vc + 4, fc, fc + 4, a.do_fej, R_C, vcal + 4, cam, pf, pff, a.uv[2 * (m0 + k)], a.uv[2 * (m0 + k) + 1], white_px,
                  res, Hf, Hcl, Hcal, Hin);
     for (int i = 0; i < 2; i++) {
       int r = 2 * k + i;
@@ -350,15 +354,16 @@ __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
     }
   } else {
     // ---- SLAM landmark: no nullspace; gate with the plane constraint, on failure retry without it (UpdaterSLAM.cpp:528-622) ----
+    // (an ArUco tag gates both tries with its own chi2_multipler, :545-547)
     double chi2 = gate_chi2(A, lda, T, S, a.ldt, vbuf, Pp, a.maxcols, 0, nr, 0, ncs, gid, a.P, a.ldP, c_res, tid, &s_ok, &s_chi2);
-    double thr = a.chi2_mult * a.chi2_table[nr < a.chi2_n ? nr : a.chi2_n - 1];
+    double thr = (TAGS ? a.feat_opt[2 * f + 1] : a.chi2_mult) * a.chi2_table[nr < a.chi2_n ? nr : a.chi2_n - 1];
     int st = (s_ok && !(chi2 > thr)) ? 1 : 0;
     if (!st && has_plane) {
       __syncthreads();
       nr = 2 * m;
       ncs = 3 + cf;
       chi2 = gate_chi2(A, lda, T, S, a.ldt, vbuf, Pp, a.maxcols, 0, nr, 0, ncs, gid, a.P, a.ldP, c_res, tid, &s_ok, &s_chi2);
-      thr = a.chi2_mult * a.chi2_table[nr < a.chi2_n ? nr : a.chi2_n - 1];
+      thr = (TAGS ? a.feat_opt[2 * f + 1] : a.chi2_mult) * a.chi2_table[nr < a.chi2_n ? nr : a.chi2_n - 1];
       st = (s_ok && !(chi2 > thr)) ? 3 : 0;
     }
     accept = st;

@@ -84,6 +84,10 @@ struct Ctx {
   std::map<int64_t, int> planes;  // State::_features_PLANE
   std::map<int64_t, int> slam;    // State::_features_SLAM
   std::map<int64_t, int64_t> slam_to_plane;
+  // UpdaterSLAM's options_aruco (ovp_set_aruco_options): with has_aruco, the SLAM entry points whiten and gate every feature with
+  // featid < opt.max_aruco_features with these instead of the call's options (aruco_options_of)
+  bool has_aruco = false;
+  ovp_updater_options aruco = {1.0, 1.0};
   std::vector<double> chi2_table;
   double *d_chi2_table = nullptr;
   int chi2_table_n = 0;
@@ -272,6 +276,13 @@ static inline Ctx *enter(ovp_ctx *h) {
 static inline bool is_clone(const Ctx *c, int h, bool need_slot) {
   return h >= 0 && h < (int)c->vars.size() && c->vars[h].alive && c->vars[h].kind == OVP_KIND_POSE && h != c->h_calib &&
          (!need_slot || c->vars[h].id >= 0);
+}
+
+// an ArUco tag corner of UpdaterSLAM ((int)featid < max_aruco_features, UpdaterSLAM.cpp:164, 257, 303, 500, 546) while ArUco options are set
+static inline bool is_aruco_tag(const Ctx *c, int64_t featid) { return c->has_aruco && (int)featid < c->opt.max_aruco_features; }
+// the options UpdaterSLAM whitens and gates feature featid with: options_aruco for a tag, the call's own (options_slam) otherwise
+static inline const ovp_updater_options &slam_options_of(const Ctx *c, int64_t featid, const ovp_updater_options &opt) {
+  return is_aruco_tag(c, featid) ? c->aruco : opt;
 }
 
 // bump allocator of a staging buffer: consecutive slices, each starting 16-byte aligned

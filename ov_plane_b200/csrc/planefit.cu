@@ -420,6 +420,7 @@ struct PoArgs {
   const float *uvn;
   const double *p0, *cp0, *Rc, *pc; // camera pose table by clone handle (cam_pose_kernel)
   double sigma_px_norm, sigma_c;
+  const double *sigma_px_norm_of; // optimize_plane_kernel<true>: problem p (block p) takes sigma_px_norm_of[p] instead of sigma_px_norm
   int max_iter;
   double R_cur[9], p_cur[3]; // current camera pose R_GtoC, p_CinG (for the in-front-of-camera test, :471-474)
   double *scratch;           // PO_FIELDS per feature
@@ -433,12 +434,13 @@ struct PoArgs {
 // lanes: U (6, packed lower), W (9), bf (3): feature blocks; Vf (6), bcf (3): this feature's share of the plane block.
 // Loss: Cauchy a = 1 on every residual block (PlaneFitting.cpp:252,363): rho = log(1 + s); corrector.cc with rho'' <= 0: residual and
 // Jacobian are scaled by sqrt(rho') = 1 / sqrt(1 + s).
+template <bool PER_PROBLEM_SIGMA>
 __device__ double po_feature_warp(const PoArgs &A, int fg, const double *p, const double *nrm, double d, bool cp_free, bool feat_free, bool want,
                                   double *U, double *W, double *bf, double *Vf, double *bcf) {
   const int lane = threadIdx.x & 31;
   const int m0 = A.meas_offset[fg], m = A.meas_offset[fg + 1] - m0;
   double part[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0}; // cost, U (6), bf (3) of this lane's measurements
-  const double w = 1.0 / A.sigma_px_norm;
+  const double w = 1.0 / (PER_PROBLEM_SIGMA ? A.sigma_px_norm_of[blockIdx.x] : A.sigma_px_norm);
   for (int k = lane; k < m; k += 32) {
     const int hc = A.meas_clone[m0 + k];
     const double *R = A.Rc + 9 * (size_t)hc, *pc = A.pc + 3 * (size_t)hc;
@@ -513,7 +515,9 @@ __device__ double po_feature_warp(const PoArgs &A, int fg, const double *p, cons
   return cost;
 }
 
-__global__ void __launch_bounds__(PO_THREADS) optimize_plane_kernel(PoArgs A) {
+// PER_PROBLEM_SIGMA: problem p takes A.sigma_px_norm_of[p]; the instantiation without it is the kernel every caller but an ArUco tag's
+// refinement runs, compiled as if the per-problem array did not exist
+template <bool PER_PROBLEM_SIGMA> __global__ void __launch_bounds__(PO_THREADS) optimize_plane_kernel(PoArgs A) {
   __shared__ double red[(PO_THREADS / 32) * 12];
   const int plane = blockIdx.x, f0 = A.feat_offset[plane], F = A.feat_offset[plane + 1] - f0, tid = threadIdx.x;
   const bool fix_plane = A.fix_plane[plane] != 0, cp_free = !fix_plane;
@@ -567,7 +571,7 @@ __global__ void __launch_bounds__(PO_THREADS) optimize_plane_kernel(PoArgs A) {
       const bool ff = A.meas_offset[f0 + f + 1] > A.meas_offset[f0 + f];
       const double p[3] = {FLD(PO_X, f, 0), FLD(PO_X, f, 1), FLD(PO_X, f, 2)};
       double U[6], W[9], bf[3], Vf[6], bcf[3];
-      const double cf = po_feature_warp(A, f0 + f, p, nrm, d, cp_free, ff, true, U, W, bf, Vf, bcf);
+      const double cf = po_feature_warp<PER_PROBLEM_SIGMA>(A, f0 + f, p, nrm, d, cp_free, ff, true, U, W, bf, Vf, bcf);
       if (lane == 0) {
         acc[0] += cf;
         for (int i = 0; i < 6; i++) {
@@ -900,7 +904,7 @@ __global__ void __launch_bounds__(PO_THREADS) optimize_plane_kernel(PoArgs A) {
         for (int f = warp; f < F; f += nwarps) {
           const bool ff = A.meas_offset[f0 + f + 1] > A.meas_offset[f0 + f];
           const double p[3] = {FLD(PO_CAND, f, 0), FLD(PO_CAND, f, 1), FLD(PO_CAND, f, 2)};
-          const double cf = po_feature_warp(A, f0 + f, p, nrm, d, cp_free, ff, false, nullptr, nullptr, nullptr, nullptr, nullptr);
+          const double cf = po_feature_warp<PER_PROBLEM_SIGMA>(A, f0 + f, p, nrm, d, cp_free, ff, false, nullptr, nullptr, nullptr, nullptr, nullptr);
           if (lane == 0)
             cc[0] += cf;
         }
@@ -1118,9 +1122,11 @@ struct RefineOut {
 };
 // optimize_plane_kernel on n_planes planes, inputs on the device as ovp_optimize_plane takes them, camera poses from t.  The current camera
 // pose of the in-front-of-camera test (stateI, calib0: PlaneFitting.cpp:441-450) comes from the host mirror: sync_host_values first.
+// sigma_px_norm_of (device, optional): a sigma_px_norm per plane problem instead of the one of the launch (an ArUco tag's in
+// ovp_slam_delayed_init_tracks).
 static int launch_optimize_plane(Ctx *c, int n_planes, const int *feat_offset, const int *meas_offset, const int *meas_clone, const float *uvn,
                                  const double *p0, const double *cp0, const int *fix_plane, double sigma_px_norm, double sigma_c, int max_iter,
-                                 char *d, const PoseTable &t, const RefineOut &o) {
+                                 char *d, const PoseTable &t, const RefineOut &o, const double *sigma_px_norm_of = nullptr) {
   PoArgs A;
   const double *vi = c->h_val.data() + (size_t)c->h_imu * OVP_VAL_STRIDE, *vc = c->h_val.data() + (size_t)c->h_calib * OVP_VAL_STRIDE;
   double Ri[9], RC[9];
@@ -1139,6 +1145,7 @@ static int launch_optimize_plane(Ctx *c, int n_planes, const int *feat_offset, c
   A.Rc = (const double *)(d + t.R);
   A.pc = (const double *)(d + t.p);
   A.sigma_px_norm = sigma_px_norm;
+  A.sigma_px_norm_of = sigma_px_norm_of;
   A.sigma_c = sigma_c;
   A.max_iter = max_iter;
   A.scratch = (double *)(d + o.scratch);
@@ -1147,7 +1154,10 @@ static int launch_optimize_plane(Ctx *c, int n_planes, const int *feat_offset, c
   A.info = (double *)(d + o.info);
   A.inlier = (int *)(d + o.inlier);
   A.status = (int *)(d + o.status);
-  optimize_plane_kernel<<<n_planes, PO_THREADS, 0, c->stream>>>(A);
+  if (sigma_px_norm_of)
+    optimize_plane_kernel<true><<<n_planes, PO_THREADS, 0, c->stream>>>(A);
+  else
+    optimize_plane_kernel<false><<<n_planes, PO_THREADS, 0, c->stream>>>(A);
   c->launches++;
   OVP_CUDA(cudaGetLastError());
   return OVP_OK;
