@@ -48,6 +48,30 @@ struct Flat { // SoA view of a feature list (mono camera)
 } // namespace
 
 // ---- UpdaterSLAM ----------------------------------------------------------------------------------------------------------------------
+namespace {
+// StateOptions::feat_rep_slam / feat_rep_aruco, host-only: the representation every new landmark is created in (UpdaterSLAM.cpp:231-232)
+void set_landmark_options(const std::shared_ptr<State> &state) {
+  const ovp_landmark_options lo = {(int)state->_options.feat_rep_slam, (int)state->_options.feat_rep_aruco};
+  ck(state->ctx, ovp_set_landmark_options(state->ctx, &lo));
+}
+// Landmark::_feat_representation, _anchor_cam_id and _anchor_clone_timestamp, value and first estimate of the landmark of featid as the
+// library holds them (the anchor's timestamp is the one of the clone whose handle the library names)
+void refresh_landmark(const std::shared_ptr<State> &state, ov_type::Landmark &landmark) {
+  int rep = 0, anchor = -1;
+  ck(state->ctx, ovp_slam_get_representation(state->ctx, (int64_t)landmark._featid, &rep, &anchor));
+  landmark._feat_representation = (ov_type::LandmarkRepresentation::Representation)rep;
+  landmark._anchor_cam_id = anchor >= 0 ? 0 : -1; // mono
+  landmark._anchor_clone_timestamp = -1;
+  for (const auto &clone : state->_clones_IMU)
+    if (anchor >= 0 && state->handle.at(clone.second.get()) == anchor)
+      landmark._anchor_clone_timestamp = clone.first;
+  Eigen::MatrixXd value(3, 1), fej(3, 1);
+  ck(state->ctx, ovp_var_get(state->ctx, state->handle.at(&landmark), value.data(), fej.data()));
+  landmark.set_value(value);
+  landmark.set_fej(fej);
+}
+} // namespace
+
 UpdaterSLAM::UpdaterSLAM(UpdaterOptions &options_slam, UpdaterOptions &options_aruco, ov_core::FeatureInitializerOptions &feat_init_options)
     : _options_slam(options_slam), _options_aruco(options_aruco) {
   (void)feat_init_options;
@@ -64,6 +88,7 @@ void UpdaterSLAM::update(std::shared_ptr<State> state, std::vector<std::shared_p
   // no state to hand them to
   const ovp_updater_options ua = {_options_aruco.sigma_pix, _options_aruco.chi2_multipler};
   ck(state->ctx, ovp_set_aruco_options(state->ctx, &ua));
+  set_landmark_options(state); // each landmark is updated in its own representation and anchor (:476-522)
   ovp_updater_options uo = {_options_slam.sigma_pix, _options_slam.chi2_multipler};
   std::vector<int> st(feature_vec.size());
   std::vector<double> chi(feature_vec.size());
@@ -85,6 +110,7 @@ void UpdaterSLAM::delayed_init(std::shared_ptr<State> state, std::vector<std::sh
   // ArUco features (featid < max_aruco_features) are initialised with _options_aruco (:164, :257, :302-304), in the same call as the rest
   const ovp_updater_options ua = {_options_aruco.sigma_pix, _options_aruco.chi2_multipler};
   ck(state->ctx, ovp_set_aruco_options(state->ctx, &ua));
+  set_landmark_options(state); // anchored landmarks are created from the triangulation's p_FinA (:230-304)
   // :77-103 clean every track against the clone times
   std::vector<double> clonetimes;
   for (const auto &clone_imu : state->_clones_IMU)
@@ -124,22 +150,30 @@ void UpdaterSLAM::delayed_init(std::shared_ptr<State> state, std::vector<std::sh
       state->_features_SLAM_to_PLANE[f->featid] = (size_t)s2p;
     if (feat_status[i] <= 0)
       continue; // erased from feature_vec
-    // :305, :352 register the landmark with the value and first estimate the device holds
+    // :283-305, :352 register the landmark with its representation, anchor, value and first estimate as the library holds them
     auto landmark = std::make_shared<ov_type::Landmark>(3);
-    Eigen::MatrixXd value(3, 1), fej(3, 1);
-    ck(state->ctx, ovp_var_get(state->ctx, new_handles[i], value.data(), fej.data()));
     landmark->_featid = f->featid;
-    landmark->set_value(value);
-    landmark->set_fej(fej);
-    state->_features_SLAM.insert({f->featid, landmark});
+    landmark->_unique_camera_id = 0;
     state->handle[landmark.get()] = new_handles[i];
+    refresh_landmark(state, *landmark);
+    state->_features_SLAM.insert({f->featid, landmark});
     state->by_handle[new_handles[i]] = landmark;
     kept.push_back(f);
   }
   feature_vec.swap(kept);
 }
 
-void UpdaterSLAM::change_anchors(std::shared_ptr<State> state) { ck(state->ctx, ovp_slam_change_anchors(state->ctx, nullptr)); }
+void UpdaterSLAM::change_anchors(std::shared_ptr<State> state) {
+  // :684-704; the landmarks the library moved get their new anchor, value and first estimate (perform_anchor_change, :840-848).  Refreshing
+  // every anchored landmark reads back, for one that did not move, what it already holds.
+  int n_changed = 0;
+  ck(state->ctx, ovp_slam_change_anchors(state->ctx, &n_changed));
+  if (n_changed == 0)
+    return;
+  for (auto &kv : state->_features_SLAM)
+    if (ov_type::LandmarkRepresentation::is_relative_representation(kv.second->_feat_representation))
+      refresh_landmark(state, *kv.second);
+}
 
 // ---- UpdaterPlane ---------------------------------------------------------------------------------------------------------------------
 UpdaterPlane::UpdaterPlane(UpdaterOptions &options, ov_core::FeatureInitializerOptions &feat_init_options) : _options(options) { (void)feat_init_options; }

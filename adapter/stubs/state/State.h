@@ -12,6 +12,8 @@ struct StateOptions {
   int max_clone_size = 11;
   int max_aruco_features = 1024;
   bool do_calib_camera_timeoffset = false;
+  ov_type::LandmarkRepresentation::Representation feat_rep_slam = ov_type::LandmarkRepresentation::GLOBAL_3D; // StateOptions.h:82-88
+  ov_type::LandmarkRepresentation::Representation feat_rep_aruco = ov_type::LandmarkRepresentation::GLOBAL_3D;
   // StateOptions.h:96-150 (plane options the updaters read)
   bool use_plane_constraint = true, use_plane_constraint_msckf = true, use_plane_constraint_slamu = true,
        use_plane_constraint_slamd = true, use_refine_plane_feat = true;

@@ -39,10 +39,30 @@ public:
 private:
   std::shared_ptr<PoseJPL> _pose;
 };
+class LandmarkRepresentation { // types/LandmarkRepresentation.h
+public:
+  enum Representation {
+    GLOBAL_3D,
+    GLOBAL_FULL_INVERSE_DEPTH,
+    ANCHORED_3D,
+    ANCHORED_FULL_INVERSE_DEPTH,
+    ANCHORED_MSCKF_INVERSE_DEPTH,
+    ANCHORED_INVERSE_DEPTH_SINGLE,
+    UNKNOWN
+  };
+  static bool is_relative_representation(Representation feat_representation) {
+    return feat_representation == ANCHORED_3D || feat_representation == ANCHORED_FULL_INVERSE_DEPTH ||
+           feat_representation == ANCHORED_MSCKF_INVERSE_DEPTH || feat_representation == ANCHORED_INVERSE_DEPTH_SINGLE;
+  }
+};
 class Landmark : public Vec {
 public:
   explicit Landmark(int dim) : Vec(dim) {}
   size_t _featid = 0;
+  int _unique_camera_id = -1;
+  int _anchor_cam_id = -1;
+  double _anchor_clone_timestamp = -1;
   bool should_marg = false;
+  LandmarkRepresentation::Representation _feat_representation = LandmarkRepresentation::UNKNOWN;
 };
 } // namespace ov_type

@@ -218,7 +218,8 @@ int ovp_msckf_update_landmarks(ovp_ctx *ctx, const ovp_feature_batch *batch, con
  * removes the features of initialised planes from its MSCKF list like UpdaterPlane.cpp:459-475. */
 int ovp_plane_init(ovp_ctx *ctx, const ovp_feature_batch *batch, const ovp_updater_options *opt, int *plane_status, int *new_handles);
 
-/* ---- UpdaterSLAM (update/UpdaterSLAM.cpp) — GLOBAL_3D landmarks, mono camera ----------------------------------------- */
+/* ---- UpdaterSLAM (update/UpdaterSLAM.cpp) — GLOBAL_3D landmarks, and with ovp_set_landmark_options the other four
+ * representations, mono camera ---------------------------------------------------------------------------------------------------------- */
 /* UpdaterSLAM::update from "calculate the max possible measurement size" on (:389-735): per landmark feature
  * get_feature_jacobian_full with the landmark (and its in-state plane, when use_plane_constraint and
  * _features_SLAM_to_PLANE allows it) as state columns, chi2 gate against the marginal covariance, on failure WITH a plane
@@ -249,6 +250,26 @@ int64_t ovp_slam_plane_of(ovp_ctx *ctx, int64_t featid); /* State::_features_SLA
  * them (the default: every feature takes the call's options, and ovp_slam_delayed_init_tracks refuses ArUco ids).  sigma_pix <= 0 or
  * chi2_multipler <= 0: OVP_ERR_BAD_ARGS, the options held before are kept.  Host-only: nothing is copied to the device. */
 int ovp_set_aruco_options(ovp_ctx *ctx, const ovp_updater_options *aruco);
+/* StateOptions::feat_rep_slam / feat_rep_aruco (state/StateOptions.h; UpdaterSLAM.cpp:231-232), numbered as in
+ * ovp_feature_jacobian_representation, 0..4.  A feature takes feat_rep_aruco when featid < max_aruco_features, feat_rep_slam otherwise.
+ * Once set:
+ *  - ovp_slam_update takes landmarks in any of the five representations, each with its own anchor (ovp_slam_get_representation), in one
+ *    batch (:476-522, UpdaterHelper.cpp:243-303, 411-420).  A landmark outside GLOBAL_3D that would take its in-state plane
+ *    (use_plane_constraint, plane in the state, _features_SLAM_to_PLANE not 0) is refused with OVP_ERR_BAD_ARGS before anything is copied or
+ *    launched: the reference's plane constraint asserts GLOBAL_3D (UpdaterHelper.cpp:455-456).  The track limit of such a batch is the
+ *    same 29 measurements, the anchor's 6 columns included (a longer track: OVP_ERR_CAPACITY before anything is launched).
+ *  - ovp_slam_delayed_init_tracks creates each landmark in its feature's representation, anchored (2..4) in the clone of the track's last
+ *    measurement (camera 0), from the triangulation's p_FinA (:230-304).  A feature outside GLOBAL_3D that would be a plane candidate is
+ *    refused up front, as above.
+ *  - ovp_slam_delayed_init, which takes p_FinG only, refuses a batch in which any feature takes another representation than GLOBAL_3D.
+ * Options {0, 0} behave exactly as none.  NULL clears them (the default: only GLOBAL_3D landmarks are created, and ovp_slam_update refuses
+ * any other).  A value outside 0..4 is OVP_ERR_BAD_ARGS, the options held before are kept; 5 (ANCHORED_INVERSE_DEPTH_SINGLE) is not
+ * supported.  Host-only: nothing is copied to the device. */
+typedef struct ovp_landmark_options {
+  int feat_rep_slam;
+  int feat_rep_aruco;
+} ovp_landmark_options;
+int ovp_set_landmark_options(ovp_ctx *ctx, const ovp_landmark_options *o);
 
 /* ---- Anchored landmark representations (UpdaterHelper.cpp:35-193, UpdaterSLAM.cpp:684-850) -------------------------------------------- */
 /* get_feature_jacobian_full (UpdaterHelper.cpp:195-449) for any ov_type::LandmarkRepresentation (numbering as in
@@ -260,8 +281,8 @@ int ovp_feature_jacobian_full_rep(ovp_ctx *ctx, int m, const int *clone_handles,
                                   const double *p_F, const double *p_F_fej, double sigma_px, double *H_f, int *hf_cols, double *H_x, int *hx_cols,
                                   double *res, int *rows_out, int *x_order, int *x_order_n);
 /* Landmark::_feat_representation / _anchor_clone_timestamp of a landmark that is in the state: declares how its 3-vector value is read
- * (0 / 2 position, 1 / 3 [theta, phi, rho], 4 [x/z, y/z, 1/z]).  The fused update entry points (ovp_slam_update, ...) are GLOBAL_3D and
- * refuse landmarks declared otherwise. */
+ * (0 / 2 position, 1 / 3 [theta, phi, rho], 4 [x/z, y/z, 1/z]).  ovp_slam_update takes landmarks declared otherwise once landmark options
+ * are set (ovp_set_landmark_options) and refuses them before; ovp_msckf_update_landmarks takes GLOBAL_3D landmarks only. */
 int ovp_slam_set_representation(ovp_ctx *ctx, int64_t featid, int representation, int anchor_clone_handle);
 int ovp_slam_get_representation(ovp_ctx *ctx, int64_t featid, int *representation, int *anchor_clone_handle);
 /* UpdaterSLAM::perform_anchor_change (:706-850): re-express an anchored landmark in another clone's camera frame; covariance through
@@ -423,10 +444,14 @@ typedef struct ovp_slam_init_options {
  * had one), 3 initialised after its plane was dropped for chi2.  plane_status[F] (may be NULL): -1 not a refinement candidate, 1 refined
  * onto its plane, 0 refinement failed.  p_FinG_out[3F]: what the reference leaves in Feature::p_FinG (the refined position for a refined
  * feature, also for status 3, whose landmark holds the triangulated one; zero for -1).  new_handles[F]: the landmark's handle, or -1.
- * Only GLOBAL_3D landmarks are created.
+ * Without landmark options only GLOBAL_3D landmarks are created.  With them (ovp_set_landmark_options) each landmark is created in its
+ * feature's representation: 2..4 anchored in the clone of the track's last measurement with the value and first estimate set_from_xyz of
+ * the triangulation's p_FinA, 1 from p_FinG, with the Jacobians of ovp_feature_jacobian_full_rep (ovp_slam_get_representation reads both).
  * Refused before anything is copied or launched, with the state untouched: a null pointer, malformed tracks (the per-track rules for the
  * tracks of two or more measurements), a duplicate featid, a featid that already has a landmark (OVP_ERR_ALREADY_IN_STATE), a featid below
- * max_aruco_features while no ArUco options are set (ovp_set_aruco_options; with them tags are accepted), a chi2 table too short for the
+ * max_aruco_features while no ArUco options are set (ovp_set_aruco_options; with them tags are accepted), a feature outside GLOBAL_3D that
+ * would be a refinement or plane candidate (use_plane_constraint, its plane in the state, _features_SLAM_to_PLANE absent or not 0: the
+ * reference asserts GLOBAL_3D there, UpdaterHelper.cpp:455-456), a chi2 table too short for the
  * rows of a feature (3 per measurement with a plane, 2 without), sigma_pix <= 0, and OVP_ERR_CAPACITY for a track longer than
  * OVP_SLAM_INIT_MAX_TRACK (64).  The state and row capacities of an initialisation depend on which features pass and are checked per
  * feature as in ovp_slam_delayed_init: such a refusal comes after the launches and keeps the landmarks initialised before it. */

@@ -42,6 +42,10 @@ class UpdaterOptions(C.Structure):
     _fields_ = [("sigma_pix", C.c_double), ("chi2_multipler", C.c_double)]
 
 
+class LandmarkOptions(C.Structure):
+    _fields_ = [("feat_rep_slam", C.c_int), ("feat_rep_aruco", C.c_int)]
+
+
 class PlaneFitOptions(C.Structure):
     _fields_ = [("min_inlier_num", C.c_int), ("max_cond_number", C.c_double), ("shuffle_kind", C.c_int)]
 
@@ -511,6 +515,16 @@ class Context(object):
             return
         uo = UpdaterOptions(float(sigma_pix), float(chi2_mult))
         self._ck(self.lib.ovp_set_aruco_options(self.h, C.byref(uo)))
+
+    def set_landmark_options(self, feat_rep_slam, feat_rep_aruco=None):
+        """StateOptions::feat_rep_slam / feat_rep_aruco (0..4, numbered as in feature_jacobian_representation; feat_rep_aruco defaults to
+        feat_rep_slam): slam_update then takes landmarks in any representation, and slam_delayed_init_tracks creates each landmark in its
+        feature's (include/ovp.h ovp_set_landmark_options).  feat_rep_slam=None clears them: only GLOBAL_3D landmarks again."""
+        if feat_rep_slam is None:
+            self._ck(self.lib.ovp_set_landmark_options(self.h, None))
+            return
+        lo = LandmarkOptions(int(feat_rep_slam), int(feat_rep_slam if feat_rep_aruco is None else feat_rep_aruco))
+        self._ck(self.lib.ovp_set_landmark_options(self.h, C.byref(lo)))
 
     def slam_handle(self, featid):
         return self.lib.ovp_slam_handle(self.h, C.c_int64(int(featid)))

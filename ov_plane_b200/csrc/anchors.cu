@@ -8,8 +8,12 @@
 //   ovp_slam_set_representation / ovp_slam_get_representation : Landmark::_feat_representation + _anchor_clone_timestamp of a landmark in the state.
 //   ovp_slam_perform_anchor_change / ovp_slam_change_anchors : the anchor-change Jacobian Phi (3 x [old anchor, extrinsics, new anchor, landmark]) on
 //       the host, StateHelper::EKFPropagation on the device (ovp_ekf_propagation), new value / first estimate of the landmark.
-// The FUSED update kernels (ovp_msckf_update, ovp_slam_update, ovp_slam_delayed_init) remain GLOBAL_3D like every shipped configuration
-// (config/*/estimator_config.yaml feat_rep_*: GLOBAL_3D; the plane constraint asserts it, UpdaterHelper.cpp:455-456) and refuse anchored landmarks.
+//   ovp_set_landmark_options : StateOptions::feat_rep_slam / feat_rep_aruco.  Once set, ovp_slam_update takes landmarks in representations 0..4
+//       (feature_kernel<true, true>, features.cu: the same chain rule on the device, its terms from the device value table) and
+//       ovp_slam_delayed_init_tracks creates them (slam_delayed_init_core, through stage_feature_jacobian_rep below).
+// Out of scope: ANCHORED_INVERSE_DEPTH_SINGLE in the state (the landmark would carry its initial bearing and the update would need a second
+// projection); the MSCKF entry points (ovp_msckf_update, ovp_msckf_update_landmarks) stay GLOBAL_3D as the reference asserts
+// (UpdaterMSCKF.cpp:250, 662), and so does any landmark on an in-state plane (the plane constraint asserts it, UpdaterHelper.cpp:455-456).
 namespace ovp {
 
 // per row r of the 2m bearing rows: raw = Hf[r, 0:3] (= w dz/dp_FinG); Hf[r, 0:k] = raw L; Hx[r, anchor cols] += raw Ha; Hx[r, calib cols] += raw Hc
@@ -96,22 +100,17 @@ static void inverse3(const double *A, double *Ai) { // column-major 3x3, Gauss-J
 }
 static bool is_relative(int rep) { return rep >= 2 && rep <= 5; }
 
-} // namespace ovp
-
-extern "C" {
-
-int ovp_feature_jacobian_full_rep(ovp_ctx *h, int m, const int *clone_handles, const float *uv, int representation, int anchor_clone_handle,
-                                  const double *p_F, const double *p_F_fej, double sigma_px, double *H_f, int *hf_cols, double *H_x, int *hx_cols,
-                                  double *res, int *rows_out, int *x_order, int *x_order_n) {
-  using namespace ovp;
-  Ctx *c = ovp::enter(h);
-  if (representation < 0 || representation > 5 || !p_F || !p_F_fej || !H_f || !H_x || !res)
-    return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full_rep: bad representation / null argument");
+// get_feature_jacobian_full of one feature in representation rep on the staging buffer (FeatureJacobianStage layout, H_f with *k columns):
+// the bearing rows of stage_feature_jacobian at p_FinG, then representation_chain_kernel (UpdaterHelper.cpp:411-420) with the 3x3 terms of
+// ovp_feature_jacobian_representation on the host values.  p_F / p_F_fej: p_FinG and its first estimate for reps 0 / 1, p_FinA for the
+// anchored ones.  *extra = 6 when no measurement was taken from the anchor: its columns follow the clones' in H_x.  dev: as for
+// stage_feature_jacobian.  Shared by ovp_feature_jacobian_full_rep and the initialisations of slam_delayed_init_core.
+static int stage_feature_jacobian_rep(Ctx *c, int m, const int *clone_handles, const float *uv, int representation, int anchor_clone_handle,
+                                      const double *p_F, const double *p_F_fej, double sigma_px, FeatureJacobianStage *jo, int *k_out,
+                                      int *extra_out, const DeviceTrack *dev) {
   const bool rel = is_relative(representation);
-  if (rel && !is_clone(c, anchor_clone_handle, true))
-    return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full_rep: anchor handle %d is not a clone in the state", anchor_clone_handle);
-  int st = check_jacobian_track(c, "feature_jacobian_full_rep", m, clone_handles);
-  if (st || (st = sync_host_values(c)))
+  int st = sync_host_values(c);
+  if (st)
     return st;
   double pG[3] = {p_F[0], p_F[1], p_F[2]}, pGf[3] = {p_F_fej[0], p_F_fej[1], p_F_fej[2]};
   const double *cal = c->h_val.data() + (size_t)c->h_calib * OVP_VAL_STRIDE;
@@ -140,8 +139,8 @@ int ovp_feature_jacobian_full_rep(ovp_ctx *h, int m, const int *clone_handles, c
     if (clone_handles[i] == anchor_clone_handle)
       anchor_k = i;
   const int extra = (rel && anchor_k < 0) ? 6 : 0;
-  FeatureJacobianStage j;
-  st = stage_feature_jacobian(c, m, clone_handles, uv, pG, pGf, false, -1, nullptr, nullptr, sigma_px, 1.0, &j, extra);
+  FeatureJacobianStage &j = *jo;
+  st = stage_feature_jacobian(c, m, clone_handles, uv, pG, pGf, false, -1, nullptr, nullptr, sigma_px, 1.0, &j, extra, dev);
   if (st)
     return st;
   const int ncal_pose = c->opt.do_calib_camera_pose ? 6 : 0, ncal = ncal_pose + (c->opt.do_calib_camera_intrinsics ? 8 : 0);
@@ -157,6 +156,32 @@ int ovp_feature_jacobian_full_rep(ovp_ctx *h, int m, const int *clone_handles, c
   representation_chain_kernel<<<(j.rows + 63) / 64, 64, 0, c->stream>>>(a);
   c->launches++;
   OVP_CUDA(cudaGetLastError());
+  *k_out = k;
+  *extra_out = extra;
+  return OVP_OK;
+}
+
+} // namespace ovp
+
+extern "C" {
+
+int ovp_feature_jacobian_full_rep(ovp_ctx *h, int m, const int *clone_handles, const float *uv, int representation, int anchor_clone_handle,
+                                  const double *p_F, const double *p_F_fej, double sigma_px, double *H_f, int *hf_cols, double *H_x, int *hx_cols,
+                                  double *res, int *rows_out, int *x_order, int *x_order_n) {
+  using namespace ovp;
+  Ctx *c = ovp::enter(h);
+  if (representation < 0 || representation > 5 || !p_F || !p_F_fej || !H_f || !H_x || !res)
+    return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full_rep: bad representation / null argument");
+  const bool rel = is_relative(representation);
+  if (rel && !is_clone(c, anchor_clone_handle, true))
+    return fail(c, OVP_ERR_BAD_ARGS, "feature_jacobian_full_rep: anchor handle %d is not a clone in the state", anchor_clone_handle);
+  int st = check_jacobian_track(c, "feature_jacobian_full_rep", m, clone_handles);
+  if (st)
+    return st;
+  FeatureJacobianStage j;
+  int k = 3, extra = 0;
+  if ((st = stage_feature_jacobian_rep(c, m, clone_handles, uv, representation, anchor_clone_handle, p_F, p_F_fej, sigma_px, &j, &k, &extra)))
+    return st;
   if ((st = read_feature_jacobian(c, j, k, H_f, H_x, res)))
     return st;
   *hf_cols = k;
@@ -172,6 +197,26 @@ int ovp_feature_jacobian_full_rep(ovp_ctx *h, int m, const int *clone_handles, c
   if (extra)
     x_order[no++] = anchor_clone_handle;
   *x_order_n = no;
+  return OVP_OK;
+}
+
+int ovp_set_landmark_options(ovp_ctx *h, const ovp_landmark_options *o) {
+  using namespace ovp;
+  Ctx *c = &h->c; // host-only: the update reads each landmark's representation from the host table when it stages a batch
+  if (!o) {
+    c->has_lm_rep = false;
+    return OVP_OK;
+  }
+  const int r[2] = {o->feat_rep_slam, o->feat_rep_aruco};
+  for (int i = 0; i < 2; i++) {
+    if (r[i] == 5)
+      return fail(c, OVP_ERR_BAD_ARGS, "set_landmark_options: %s = 5 (ANCHORED_INVERSE_DEPTH_SINGLE) is not supported: the landmark would have to "
+                  "carry the bearing it was initialised with", i ? "feat_rep_aruco" : "feat_rep_slam");
+    if (r[i] < 0 || r[i] > 4)
+      return fail(c, OVP_ERR_BAD_ARGS, "set_landmark_options: %s = %d is not a representation (0..4)", i ? "feat_rep_aruco" : "feat_rep_slam", r[i]);
+  }
+  c->lm_rep = *o;
+  c->has_lm_rep = true;
   return OVP_OK;
 }
 

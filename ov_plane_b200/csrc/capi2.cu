@@ -1673,14 +1673,23 @@ struct DeviceTracks {
   const int *at;
   size_t stage_base;
 };
+static bool is_relative(int rep);
+static bool landmark_set_from_xyz(int rep, const double *p, double *v);
+static int stage_feature_jacobian_rep(Ctx *c, int m, const int *clone_handles, const float *uv, int representation, int anchor_clone_handle,
+                                      const double *p_F, const double *p_F_fej, double sigma_px, FeatureJacobianStage *jo, int *k_out,
+                                      int *extra_out, const DeviceTrack *dev = nullptr); // anchors.cu
 // UpdaterSLAM::delayed_init, estimator half (UpdaterSLAM.cpp:225-372): per feature, in order, get_feature_jacobian_full with the
 // plane constraint when the plane is in the state, StateHelper::initialize(landmark, ..., chi2_multipler); when that fails WITH a
 // plane, detach the landmark from the plane and retry from the pre-refinement position (:310-359).  An ArUco tag takes the context's
-// ArUco options on both tries (slam_options_of).  Shared by ovp_slam_delayed_init
-// (dev == nullptr: each attempt stages its track from meas_clone / uv) and ovp_slam_delayed_init_tracks (uv unused).
+// ArUco options on both tries (slam_options_of).  A feature whose representation (landmark_rep_of) is not GLOBAL_3D has no plane (its
+// caller refuses it otherwise) and is initialised once, with the Jacobians of stage_feature_jacobian_rep (:230-304): anchored (2..4) in the
+// clone of its last measurement, from p_FinA (its value and first estimate are set_from_xyz(p_FinA)); rep 1 from p_FinG.  Shared by
+// ovp_slam_delayed_init (dev == nullptr: each attempt stages its track from meas_clone / uv; p_FinA == nullptr, GLOBAL_3D only) and
+// ovp_slam_delayed_init_tracks (uv unused).
 static int slam_delayed_init_core(Ctx *c, int F, const int *meas_offset, const int *meas_clone, const float *uv, const DeviceTracks *dev,
                                   const double *p_FinG, const double *p_FinG_original, const int64_t *featid, const int64_t *planeid,
-                                  const ovp_updater_options *opt, int use_plane, int *feat_status, int *new_handles) {
+                                  const ovp_updater_options *opt, int use_plane, int *feat_status, int *new_handles,
+                                  const double *p_FinA = nullptr) {
   for (int f = 0; f < F; f++) {
     feat_status[f] = 0;
     new_handles[f] = -1;
@@ -1695,6 +1704,48 @@ static int slam_delayed_init_core(Ctx *c, int F, const int *meas_offset, const i
     if (dev)
       dt = {dev->clone + dev->at[f], dev->uv + 2 * (size_t)dev->at[f], dev->stage_base};
     const ovp_updater_options &fo = slam_options_of(c, featid[f], *opt); // an ArUco tag's own (UpdaterSLAM.cpp:257, 302-304)
+    const int rep = landmark_rep_of(c, featid[f]);
+    if (rep != 0) {
+      if (ph >= 0 || (is_relative(rep) && !p_FinA)) // refused up front by both callers
+        return fail(c, OVP_ERR_BAD_ARGS, "delayed_init: feature %lld in representation %d", (long long)featid[f], rep);
+      const int anc = is_relative(rep) ? cl[m - 1] : -1; // FeatureInitializer's anchor of a mono track: the last measurement's clone
+      const double *pF = is_relative(rep) ? p_FinA + 3 * (size_t)f : p_FinG + 3 * (size_t)f;
+      FeatureJacobianStage j;
+      int k = 3, extra = 0;
+      int st = stage_feature_jacobian_rep(c, m, cl, dev ? nullptr : uv + 2 * (size_t)meas_offset[f], rep, anc, pF, pF, fo.sigma_pix, &j, &k, &extra,
+                                          dev ? &dt : nullptr);
+      if (st)
+        return st;
+      std::vector<int> xo;
+      if (c->opt.do_calib_camera_pose)
+        xo.push_back(c->h_calib);
+      if (c->opt.do_calib_camera_intrinsics)
+        xo.push_back(c->h_intr);
+      for (int i = 0; i < m; i++)
+        xo.push_back(cl[i]);
+      if (extra)
+        xo.push_back(anc);
+      int n = 0;
+      if ((st = upload_cols(c, xo.data(), (int)xo.size(), 0, &n)))
+        return st;
+      if (n != j.hxc)
+        return fail(c, OVP_ERR_BAD_ARGS, "delayed_init: internal column mismatch %d vs %d", n, j.hxc);
+      if (c->var_table_dirty && (st = upload_var_table(c)))
+        return st;
+      double v[3]; // Landmark::set_from_xyz (:283-289)
+      landmark_set_from_xyz(rep, pF, v);
+      int acc = 0, nh = -1;
+      if ((st = initialize_core(c, OVP_KIND_LANDMARK, 3, v, v, featid[f], c->dcols, n, j.W(c), j.rows, j.rows, j.rows, 1.0, fo.chi2_multipler, 1,
+                                &acc, &nh)))
+        return st;
+      if (acc) {
+        feat_status[f] = 1;
+        new_handles[f] = nh;
+        c->vars[nh].rep = rep;
+        c->vars[nh].anchor = anc;
+      }
+      continue;
+    }
     auto attempt = [&](const double *pf, int plane_h, int *acc, int *nh) -> int {
       FeatureJacobianStage j;
       int st = stage_feature_jacobian(c, m, cl, dev ? nullptr : uv + 2 * (size_t)meas_offset[f], pf, pf, plane_h >= 0, plane_h, nullptr, nullptr,
@@ -1766,6 +1817,11 @@ int ovp_slam_delayed_init(ovp_ctx *h, int F, const int *meas_offset, const int *
   int st = check_tracks(c, "slam_delayed_init", F, meas_offset, meas_clone, nullptr, 1, 64, OVP_ERR_BAD_ARGS, false, true);
   if (st)
     return st;
+  for (int f = 0; f < F; f++) // the reference initialises such a landmark from p_FinA, which this entry point does not take
+    if (landmark_rep_of(c, featid[f]) != 0)
+      return fail(c, OVP_ERR_BAD_ARGS, "slam_delayed_init: feature %lld takes representation %d (ovp_set_landmark_options); landmarks outside "
+                  "GLOBAL_3D are initialised from the triangulation's p_FinA by ovp_slam_delayed_init_tracks", (long long)featid[f],
+                  landmark_rep_of(c, featid[f]));
   return slam_delayed_init_core(c, F, meas_offset, meas_clone, uv, nullptr, p_FinG, p_FinG_original, featid, planeid, opt, use_plane_constraint,
                                 feat_status, new_handles);
 }

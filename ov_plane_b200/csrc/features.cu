@@ -64,6 +64,9 @@ struct FeatArgs {
   int lda;   // smem column stride of the feature block (odd)
   int ldt;   // smem column stride of T / S (odd)
   int maxcols; // capacity of local columns
+  // feature_kernel<true, true> (mode 2): per feature (global index) {representation, anchor clone handle, index of the measurement taken
+  // from the anchor or -1}.  Last, so that the other instantiations read every field at the offset they always had.
+  const int *feat_rep;
 };
 
 __device__ __forceinline__ double warp_sum(double s) {
@@ -163,12 +166,31 @@ __device__ double gate_chi2(const double *A, int lda, double *T, double *S, int 
 //   [0,3) H_f | [3, 3+cf) H_x = [extrinsics 6][intrinsics 8][clone_0 6]...[clone_{m-1} 6] | [3+cf, 3+cf+3) H_cp | last: res
 // TAGS (ovp_slam_update with an ArUco tag in the batch): every feature's whitening and chi2 multiplier come from a.feat_opt.  The
 // instantiation without it is the kernel of every other launch, compiled as if the per-feature options did not exist.
-template <bool TAGS> __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
+// REL (ovp_slam_update with a landmark in a representation other than GLOBAL_3D; launched with TAGS): a.feat_rep gives each landmark's
+// representation and anchor.  Thread 0 forms p_FinG and the chain terms from the value table (landmark_rep_terms); each measurement's
+// bearing rows are taken at p_FinG and chained: H_f = (w dz/dp_FinG) dpfg_dlambda, anchor clone += (w dz/dp_FinG) dpfg_danchor,
+// extrinsics += (w dz/dp_FinG) dpfg_dcalib (UpdaterHelper.cpp:281-303, 411-420).  An anchor no measurement was taken from gets a 6-column
+// block after the track's clones, so H_x = [extrinsics][intrinsics][clone_0]...[clone_{m-1}][anchor].  Such a landmark has no plane.
+template <bool TAGS, bool REL = false> __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
   extern __shared__ double sm[];
   const int tid = threadIdx.x;
   const int f = a.feat_sel[blockIdx.x];
   const int m0 = a.meas_offset[f];
   const int m = a.meas_offset[f + 1] - m0;
+  int rep = 0, anc = -1, anc_k = -1;
+  const double *rt = nullptr; // REL: landmark_rep_terms of this landmark (p_FinG, its first estimate, dpfg_dlambda, _danchor, _dcalib)
+  if constexpr (REL) {
+    __shared__ double s_rt[51];
+    rep = a.feat_rep[3 * f];
+    anc = a.feat_rep[3 * f + 1];
+    anc_k = a.feat_rep[3 * f + 2];
+    if (rep != 0 && tid == 0)
+      landmark_rep_terms(rep, a.do_fej, a.val + (size_t)a.feat_lm[f] * OVP_VAL_STRIDE, a.fej + (size_t)a.feat_lm[f] * OVP_VAL_STRIDE,
+                         a.val + (size_t)(anc >= 0 ? anc : 0) * OVP_VAL_STRIDE, a.fej + (size_t)(anc >= 0 ? anc : 0) * OVP_VAL_STRIDE,
+                         a.val + (size_t)a.h_calib * OVP_VAL_STRIDE, s_rt);
+    rt = s_rt; // published by the barrier after the block is cleared
+  }
+  const int xa = (REL && rep >= 2 && anc_k < 0) ? 6 : 0; // the anchor's own columns
   if (a.mode == 0) {
     int slot = a.feat_plane_slot[f];
     if (slot >= 0 && a.plane_pass[slot] == 1) { // consumed by a successful plane update (UpdaterMSCKF.cpp:640-644,659)
@@ -183,7 +205,7 @@ template <bool TAGS> __global__ void __launch_bounds__(128) feature_kernel(FeatA
   const int ph = (a.mode == 2) ? a.feat_ph[f] : a.plane_handle;
   const bool has_plane = (a.mode == 1) || (a.mode == 2 && ph >= 0);
   const int ncal = (a.do_calib_pose ? 6 : 0) + (a.do_calib_intr ? 8 : 0);
-  const int cf = ncal + 6 * m;
+  const int cf = ncal + 6 * m + xa;
   const int rows = has_plane ? 3 * m : 2 * m;
   const int ncols = 3 + cf + 3 + 1;
   const int c_cp = 3 + cf, c_res = 3 + cf + 3;
@@ -193,7 +215,7 @@ template <bool TAGS> __global__ void __launch_bounds__(128) feature_kernel(FeatA
   double *S = T + (size_t)a.ldt * 8;                // ldt * ldt         (gate only)
   double *vbuf = (a.mode == 1) ? T : S + (size_t)a.ldt * a.ldt; // reflector / forward-substitution vector
   double *Pp = vbuf + lda + 1;                                 // 8 x maxcols covariance panel (gate only)
-  __shared__ int gid[3 + 14 + 6 * 64 + 3]; // state index of every local column except the residual
+  __shared__ int gid[3 + 14 + 6 * 64 + 3 + (REL ? 6 : 0)]; // state index of every local column except the residual
   __shared__ double s_beta, s_chi2;
   __shared__ int s_ok;
 
@@ -219,10 +241,33 @@ template <bool TAGS> __global__ void __launch_bounds__(128) feature_kernel(FeatA
       pf = a.pf + 3 * (size_t)f;
       pff = pf;
     }
+    if constexpr (REL)
+      if (rep != 0) { // p_FinG and its first estimate from the landmark's value (UpdaterSLAM.cpp:476-489, UpdaterHelper.cpp:281-303)
+        pf = rt;
+        pff = rt + 3;
+      }
     double res[2], Hf[6], Hcl[12], Hcal[12], Hin[16];
     const double white_px = TAGS ? a.feat_opt[2 * f] : a.white_px; // an ArUco tag's own sigma_pix (UpdaterSLAM.cpp:500)
     bearing_rows(vc, vc + 4, fc, fc + 4, a.do_fej, R_C, vcal + 4, cam, pf, pff, a.uv[2 * (m0 + k)], a.uv[2 * (m0 + k) + 1], white_px,
                  res, Hf, Hcl, Hcal, Hin);
+    double dz[6]; // REL: w dz/dp_FinG of the two rows, before the chain rule replaces Hf
+    if constexpr (REL)
+      if (rep != 0) {
+        const double *L = rt + 6, *Ha = rt + 15, *Hc = rt + 33;
+        for (int i = 0; i < 6; i++)
+          dz[i] = Hf[i];
+        for (int i = 0; i < 2; i++) {
+          const double *r3 = dz + 3 * i;
+          for (int j = 0; j < 3; j++)
+            Hf[3 * i + j] = r3[0] * L[3 * j] + r3[1] * L[3 * j + 1] + r3[2] * L[3 * j + 2];
+          if (rep >= 2) {
+            for (int j = 0; j < 6 && a.do_calib_pose; j++)
+              Hcal[6 * i + j] += r3[0] * Hc[3 * j] + r3[1] * Hc[3 * j + 1] + r3[2] * Hc[3 * j + 2];
+            for (int j = 0; j < 6 && anc_k == k; j++) // the measurement taken from the anchor
+              Hcl[6 * i + j] += r3[0] * Ha[3 * j] + r3[1] * Ha[3 * j + 1] + r3[2] * Ha[3 * j + 2];
+          }
+        }
+      }
     for (int i = 0; i < 2; i++) {
       int r = 2 * k + i;
       for (int j = 0; j < 3; j++)
@@ -241,6 +286,13 @@ template <bool TAGS> __global__ void __launch_bounds__(128) feature_kernel(FeatA
       for (int j = 0; j < 6; j++)
         A[(size_t)(cb + 6 * k + j) * lda + r] = Hcl[6 * i + j];
       A[(size_t)c_res * lda + r] = res[i];
+      if constexpr (REL)
+        if (rep >= 2 && anc_k != k) { // this row's share of the anchor's columns (another measurement's clone, or the anchor's own block)
+          const double *Ha = rt + 15, *r3 = dz + 3 * i;
+          double *Ac = A + (size_t)(cb + 6 * (anc_k >= 0 ? anc_k : m)) * lda + r;
+          for (int j = 0; j < 6; j++)
+            Ac[(size_t)j * lda] += r3[0] * Ha[3 * j] + r3[1] * Ha[3 * j + 1] + r3[2] * Ha[3 * j + 2];
+        }
     }
 #ifdef OVP_DEBUG
     if (a.raw) // the rows just written to A, in the layout of OVP_RAW_ROW (SLAM: [0,3) are the landmark's columns)
@@ -301,6 +353,9 @@ template <bool TAGS> __global__ void __launch_bounds__(128) feature_kernel(FeatA
       gid[j] = (lm >= 0) ? a.var_id[lm] + j : 0;
       gid[c_cp + j] = (ph >= 0) ? a.var_id[ph] + j : 0;
     }
+    if constexpr (REL)
+      for (int j = 0; j < xa; j++)
+        gid[3 + ncal + 6 * m + j] = a.var_id[anc] + j;
   }
   __syncthreads();
 

@@ -1,5 +1,6 @@
 // Per-measurement arithmetic of UpdaterHelper::get_feature_jacobian_full (UpdaterHelper.cpp:350-441, :447-512), mono camera,
-// GLOBAL_3D representation, radtan distortion (ov_core::CamRadtan — every shipped config, config/*/kalibr_imucam_chain.yaml).
+// GLOBAL_3D representation, radtan distortion (ov_core::CamRadtan — every shipped config, config/*/kalibr_imucam_chain.yaml); at the end,
+// the terms that chain the bearing rows onto a landmark held in one of the other representations (landmark_rep_terms).
 // Shared by the CUDA feature kernels and by host code of the library (camera poses in planefit.cu / anchors.cu), hence __host__ __device__.
 #pragma once
 #include <math.h>
@@ -177,6 +178,113 @@ OVP_HD void plane_row(const double *pf, const double *pf_fej, const double *cp, 
     Hcp[j] = s * (p[j] - ntp * n[j] - d * n[j]);
     Hf[j] = white_c * n[j];
   }
+}
+
+// ---- A landmark in the state in representation rep 1..4 (ov_type::LandmarkRepresentation; rep 0 needs none of this) ----
+// ov_type::Landmark::get_xyz: 1 / 3 store [theta, phi, rho] (rho = 1 / range), 4 [x/z, y/z, 1/z], 2 the position itself
+OVP_HD void landmark_xyz(int rep, const double *v, double *p) {
+  if (rep == 4) {
+    p[0] = v[0] / v[2], p[1] = v[1] / v[2], p[2] = 1.0 / v[2];
+  } else if (rep == 1 || rep == 3) {
+    p[0] = (1.0 / v[2]) * cos(v[0]) * sin(v[1]);
+    p[1] = (1.0 / v[2]) * sin(v[0]) * sin(v[1]);
+    p[2] = (1.0 / v[2]) * cos(v[1]);
+  } else {
+    p[0] = v[0], p[1] = v[1], p[2] = v[2];
+  }
+}
+// d p / d (theta, phi, rho) of p = (1 / rho) [cos(theta) sin(phi), sin(theta) sin(phi), cos(phi)], evaluated at p (row-major)
+OVP_HD void landmark_d_spherical(const double *p, double *D) {
+  const double r = sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]);
+  const double rho = 1.0 / r, phi = acos(rho * p[2]), th = atan2(p[1], p[0]);
+  const double st = sin(th), ct = cos(th), sp = sin(phi), cp = cos(phi), ir = 1.0 / rho, ir2 = 1.0 / (rho * rho);
+  const double d[9] = {-ir * st * sp, ir * ct * cp, -ir2 * ct * sp, ir * ct * sp, ir * st * cp, -ir2 * st * sp, 0.0, -ir * sp, -ir2 * cp};
+  for (int i = 0; i < 9; i++)
+    D[i] = d[i];
+}
+// The terms get_feature_jacobian_full chains onto the bearing rows of a landmark in representation rep (UpdaterHelper.cpp:35-193, 281-303,
+// 411-420), from the landmark's value lv / first estimate lf, the anchor clone's pose anc / first-estimate pose ancf (rep 2..4) and the
+// extrinsics cal (7 each, JPL quaternion then position):
+//   out[0:3]   p_FinG (rep 2..4: R_GtoI^T R_ItoC^T (p_FinA - p_IinC) + p_IinG at the anchor's current pose), out[3:6] its first estimate
+//              (the same point for rep 2..4, :301-303);
+//   out[6:15]  dpfg_dlambda, column-major 3 x 3;
+//   out[15:33] dpfg_danchor and out[33:51] dpfg_dcalib, column-major 3 x 6 (rep 2..4 only), taken at the first-estimate anchor when do_fej.
+// The same algebra as ovp_feature_jacobian_representation, written for one device thread.
+OVP_HD void landmark_rep_terms(int rep, int do_fej, const double *lv, const double *lf, const double *anc, const double *ancf,
+                               const double *cal, double *out) {
+  double *pG = out, *pGf = out + 3, *L = out + 6, *Ha = out + 15, *Hc = out + 33;
+  double D[9], M[9];
+  if (rep == 1) {
+    landmark_xyz(1, lv, pG);
+    landmark_xyz(1, lf, pGf);
+    landmark_d_spherical(do_fej ? pGf : pG, D);
+    for (int i = 0; i < 3; i++)
+      for (int j = 0; j < 3; j++)
+        L[3 * j + i] = D[3 * i + j];
+    return;
+  }
+  double RC[9], RI[9], pA[3], t[3], u[3];
+  landmark_xyz(rep, lv, pA);
+  quat_to_rot(cal, RC);
+  quat_to_rot(anc, RI);
+  for (int i = 0; i < 3; i++)
+    t[i] = pA[i] - cal[4 + i];
+  for (int i = 0; i < 3; i++)
+    u[i] = RC[i] * t[0] + RC[3 + i] * t[1] + RC[6 + i] * t[2]; // R_ItoC^T t
+  for (int i = 0; i < 3; i++)
+    pG[i] = RI[i] * u[0] + RI[3 + i] * u[1] + RI[6 + i] * u[2] + anc[4 + i];
+  for (int i = 0; i < 3; i++)
+    pGf[i] = pG[i];
+  const double *pI = anc + 4;
+  if (do_fej) { // the best global estimate seen from the first-estimate anchor frame: pA = R_ItoC R_GtoI (p_FinG - p_IinG) + p_IinC
+    quat_to_rot(ancf, RI);
+    pI = ancf + 4;
+    double g[3], w[3];
+    for (int i = 0; i < 3; i++)
+      g[i] = pG[i] - pI[i];
+    mat3_vec(RI, g, w);
+    mat3_vec(RC, w, pA);
+    for (int i = 0; i < 3; i++)
+      pA[i] += cal[4 + i];
+  }
+  double RCtoG[9], dA[3], v[3], S[9], T[9]; // R_CtoG = R_GtoI^T R_ItoC^T (row-major), dA = p_FinA - p_IinC
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++)
+      RCtoG[3 * i + j] = RI[i] * RC[3 * j] + RI[3 + i] * RC[3 * j + 1] + RI[6 + i] * RC[3 * j + 2];
+  for (int i = 0; i < 3; i++)
+    dA[i] = pA[i] - cal[4 + i];
+  for (int i = 0; i < 3; i++)
+    v[i] = RC[i] * dA[0] + RC[3 + i] * dA[1] + RC[6 + i] * dA[2]; // R_ItoC^T dA
+  skew3(v, S);
+  for (int i = 0; i < 3; i++) // dpfg_danchor[:, 0:3] = -R_GtoI^T skew(R_ItoC^T dA), [:, 3:6] = I
+    for (int j = 0; j < 3; j++) {
+      Ha[3 * j + i] = -(RI[i] * S[j] + RI[3 + i] * S[3 + j] + RI[6 + i] * S[6 + j]);
+      Ha[3 * (3 + j) + i] = (i == j) ? 1.0 : 0.0;
+    }
+  skew3(dA, S);
+  mat3_mul(RCtoG, S, T);
+  for (int i = 0; i < 3; i++) // dpfg_dcalib[:, 0:3] = -R_CtoG skew(dA), [:, 3:6] = -R_CtoG
+    for (int j = 0; j < 3; j++) {
+      Hc[3 * j + i] = -T[3 * i + j];
+      Hc[3 * (3 + j) + i] = -RCtoG[3 * i + j];
+    }
+  if (rep == 2) {
+    for (int i = 0; i < 9; i++)
+      M[i] = RCtoG[i];
+  } else {
+    if (rep == 3) {
+      landmark_d_spherical(pA, D);
+    } else { // lambda = (x/z, y/z, 1/z)
+      const double rho = 1.0 / pA[2], al = pA[0] / pA[2], be = pA[1] / pA[2], ir = 1.0 / rho, ir2 = 1.0 / (rho * rho);
+      const double d[9] = {ir, 0.0, -ir2 * al, 0.0, ir, -ir2 * be, 0.0, 0.0, -ir2};
+      for (int i = 0; i < 9; i++)
+        D[i] = d[i];
+    }
+    mat3_mul(RCtoG, D, M);
+  }
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++)
+      L[3 * j + i] = M[3 * i + j];
 }
 
 } // namespace ovp

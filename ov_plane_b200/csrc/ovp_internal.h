@@ -88,6 +88,10 @@ struct Ctx {
   // featid < opt.max_aruco_features with these instead of the call's options (aruco_options_of)
   bool has_aruco = false;
   ovp_updater_options aruco = {1.0, 1.0};
+  // StateOptions::feat_rep_slam / feat_rep_aruco (ovp_set_landmark_options): with has_lm_rep, ovp_slam_update takes landmarks in any
+  // representation 0..4 and ovp_slam_delayed_init_tracks creates each landmark in its feature's (landmark_rep_of)
+  bool has_lm_rep = false;
+  ovp_landmark_options lm_rep = {0, 0};
   std::vector<double> chi2_table;
   double *d_chi2_table = nullptr;
   int chi2_table_n = 0;
@@ -283,6 +287,13 @@ static inline bool is_aruco_tag(const Ctx *c, int64_t featid) { return c->has_ar
 // the options UpdaterSLAM whitens and gates feature featid with: options_aruco for a tag, the call's own (options_slam) otherwise
 static inline const ovp_updater_options &slam_options_of(const Ctx *c, int64_t featid, const ovp_updater_options &opt) {
   return is_aruco_tag(c, featid) ? c->aruco : opt;
+}
+// the representation UpdaterSLAM creates the landmark of feature featid in (UpdaterSLAM.cpp:231-232): feat_rep_aruco for an ArUco id,
+// feat_rep_slam otherwise; GLOBAL_3D (0) while no landmark options are set
+static inline int landmark_rep_of(const Ctx *c, int64_t featid) {
+  if (!c->has_lm_rep)
+    return 0;
+  return (int)featid < c->opt.max_aruco_features ? c->lm_rep.feat_rep_aruco : c->lm_rep.feat_rep_slam;
 }
 
 // bump allocator of a staging buffer: consecutive slices, each starting 16-byte aligned

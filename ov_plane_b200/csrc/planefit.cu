@@ -1029,17 +1029,21 @@ __global__ void cam_pose_kernel(int nh, const int *var_kind, const int *var_id, 
     pc[3 * (size_t)h + i] = v[4 + i] - (R[i] * cal[4] + R[3 + i] * cal[5] + R[6 + i] * cal[6]);
 }
 // FeatureInitializer::single_triangulation + single_gaussnewton on the device (triangulate_core.h), a thread per feature
+// p_FinA (optional): the position in the anchor camera frame as well (ovp_slam_delayed_init_tracks with anchored landmarks)
 __global__ void triangulate_kernel(int F, const int *meas_offset, const int *meas_clone, const float *uvn, const double *Rc, const double *pc,
-                                   TriOptions o, double *p_FinG, int *status) {
+                                   TriOptions o, double *p_FinG, int *status, double *p_FinA) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F)
     return;
   const int m0 = meas_offset[f], m = meas_offset[f + 1] - m0;
-  double pf[3] = {0.0, 0.0, 0.0};
-  const int ok = (m >= 2) ? triangulate_feature(m, meas_clone + m0, Rc, pc, uvn + 2 * (size_t)m0, o, pf) : 0;
+  double pf[3] = {0.0, 0.0, 0.0}, pa[3] = {0.0, 0.0, 0.0};
+  const int ok = (m >= 2) ? triangulate_feature(m, meas_clone + m0, Rc, pc, uvn + 2 * (size_t)m0, o, pf, p_FinA ? pa : nullptr) : 0;
   status[f] = ok;
   for (int i = 0; i < 3; i++)
     p_FinG[3 * (size_t)f + i] = pf[i];
+  if (p_FinA)
+    for (int i = 0; i < 3; i++)
+      p_FinA[3 * (size_t)f + i] = pa[i];
 }
 
 // the caller's options, or FeatureInitializerOptions' defaults (ov_core) when there are none
@@ -1060,11 +1064,11 @@ static void launch_cam_poses(Ctx *c, char *d, const PoseTable &t) { // launch er
   c->launches++;
 }
 
-// F tracks (meas_offset: F + 1 entries) against the pose table t -> p_FinG (F x 3), status (F)
+// F tracks (meas_offset: F + 1 entries) against the pose table t -> p_FinG (F x 3), status (F), and p_FinA (F x 3) when not null
 static int launch_triangulate(Ctx *c, int F, const int *meas_offset, const int *meas_clone, const float *uvn, const TriOptions &o, char *d,
-                              const PoseTable &t, double *p_FinG, int *status) {
+                              const PoseTable &t, double *p_FinG, int *status, double *p_FinA = nullptr) {
   triangulate_kernel<<<(F + 63) / 64, 64, 0, c->stream>>>(F, meas_offset, meas_clone, uvn, (const double *)(d + t.R), (const double *)(d + t.p), o,
-                                                          p_FinG, status);
+                                                          p_FinG, status, p_FinA);
   c->launches++;
   OVP_CUDA(cudaGetLastError());
   return OVP_OK;

@@ -60,7 +60,9 @@ OVP_HD void tri_eig_minmax(const double *A, double &emin, double &emax) {
 
 // Camera poses come from a table indexed by idx[k] for measurement k: Rc (9 each, R_GtoCi row-major) and pc (3 each, p_CiinG);
 // uvn: 2 floats per measurement.  Returns 1 and p_FinG on success; 0 when single_triangulation or single_gaussnewton would return false.
-OVP_HD int triangulate_feature(int m, const int *idx, const double *Rc, const double *pc, const float *uvn, const TriOptions &o, double *p_FinG) {
+// p_FinA (optional): the position in the anchor camera frame, written on success (FeatureInitializer's Feature::p_FinA).
+OVP_HD int triangulate_feature(int m, const int *idx, const double *Rc, const double *pc, const float *uvn, const TriOptions &o, double *p_FinG,
+                               double *p_FinA = nullptr) {
   const double *RA = Rc + 9 * idx[m - 1], *pA = pc + 3 * idx[m - 1]; // anchor = last measurement
   // ---- single_triangulation ----
   double A[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0};
@@ -199,6 +201,9 @@ OVP_HD int triangulate_feature(int m, const int *idx, const double *Rc, const do
   // p_FinG = R_GtoA^T p_FinA + p_AinG
   for (int i = 0; i < 3; i++)
     p_FinG[i] = RA[i] * pfa[0] + RA[3 + i] * pfa[1] + RA[6 + i] * pfa[2] + pA[i];
+  if (p_FinA)
+    for (int i = 0; i < 3; i++)
+      p_FinA[i] = pfa[i];
   return 1;
 }
 
