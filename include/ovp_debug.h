@@ -48,12 +48,24 @@ int ovp_debug_force_dense_features(ovp_ctx *ctx, int on);
 /* on != 0: every later compressed update of this context forms M = P[:, cols] L and S = L^T M[cols, :] + I with two GEMM launches after
  * the factorisation of its Gram matrix, instead of inside that factorisation launch */
 int ovp_debug_unfused_update_products(ovp_ctx *ctx, int on);
+/* on != 0: every later compressed update of this context factors its Gram matrix and its innovation system one after the other, also
+ * when the two fit a pair (the innovation factorisation starting while the Gram factorisation runs) */
+int ovp_debug_sequential_factorisations(ovp_ctx *ctx, int on);
 /* one factorisation of the lower triangle of G ((nc + 1) x (nc + 1), column-major) over its leading npiv columns with pivot tolerance
  * tol, forming the update products in the same launch: with L = rows [0, nc) of the factor, M = P[:, cols] L (N x npiv) and the lower
  * tiles of S = L^T M[cols, :] + I (npiv x npiv; the 64 x 64 tiles on and below the diagonal are written, S_out's other entries are kept).  P is N x N, cols holds nc indices into it.
  * L_out receives the factor's (nc + 1) x npiv columns. */
 int ovp_debug_chol_products(ovp_ctx *ctx, const double *G, int nc, int npiv, double tol, const double *P, int N, const int *cols,
                             double *L_out, double *M_out, double *S_out);
+/* ovp_debug_chol_products followed by the innovation factorisation of the compressed update, as the update runs them (as a pair when
+ * they fit co-resident together and ovp_debug_sequential_factorisations is off, else one after the other): with z = row nc of the Gram
+ * factor, S = L_S L_S^T (LS_out: S's lower tiles on input as S_out above, the factor on output), Y = M L_S^-T (Y_out, N x npiv),
+ * w = L_S^-1 z (w_out), chi2 = |w|^2 (chi2_out) and the gate (gate_out: 1 when gate_thresh < 0 or chi2 <= gate_thresh).  info[0] = 1 when
+ * the pair ran.  timeline (NULL or 64 doubles, debug stamps of the pair, us from the first, -1 where absent): [k] the
+ * Gram spine released its diagonal block k, [32 + k] the innovation spine started step k. */
+int ovp_debug_chol_pair(ovp_ctx *ctx, const double *G, int nc, int npiv, double tol, const double *P, int N, const int *cols,
+                        double gate_thresh, double *L_out, double *M_out, double *LS_out, double *Y_out, double *w_out, double *chi2_out,
+                        int *gate_out, int *info, double *timeline);
 /* prepare a feature batch as ovp_msckf_update does and run the first non-empty plan of its launch order (planes in ascending id, then the
  * point update) up to its Gram matrix G = [H_o r_o]^T [H_o r_o] of the nullspace-projected system; the state is left as it was.  G_out
  * (gcap * gcap doubles) receives all of G, nc1 x nc1 column-major: the ncx x columns (calibration, then 6 per clone), for a plane its

@@ -336,10 +336,20 @@ int ovp_create(const ovp_state_options *opt, int device, int max_state, int max_
   OVP_CUDA(cudaMalloc(&c->cf_diag0, (size_t)c->cf_maxT * 64 * sizeof(double)));
   OVP_CUDA(cudaMemset(c->cf_diag0, 0, (size_t)c->cf_maxT * 64 * sizeof(double)));
   OVP_CUDA(cudaMalloc(&c->cf_flags, (size_t)(3 * c->cf_maxT + c->cf_maxT * c->cf_maxT) * sizeof(int)));
-  OVP_CUDA(cudaMalloc(&c->cf_ctrl, (4 + c->cf_maxT) * sizeof(int))); // epoch, finished CTAs, product queue head, M done per column block
+  // epoch, finished CTAs, product queue head, M done per column block, z-row tiles stored, "S(i, j) stored" per lower tile
+  const size_t nctrl = 5 + c->cf_maxT + (size_t)c->cf_maxT * (c->cf_maxT + 1) / 2;
+  OVP_CUDA(cudaMalloc(&c->cf_ctrl, nctrl * sizeof(int)));
   OVP_CUDA(cudaMemset(c->cf_linv, 0, (size_t)c->cf_maxT * 4096 * sizeof(double)));
   OVP_CUDA(cudaMemset(c->cf_flags, 0, (size_t)(3 * c->cf_maxT + c->cf_maxT * c->cf_maxT) * sizeof(int)));
-  OVP_CUDA(cudaMemset(c->cf_ctrl, 0, (4 + c->cf_maxT) * sizeof(int)));
+  OVP_CUDA(cudaMemset(c->cf_ctrl, 0, nctrl * sizeof(int)));
+  // the second set, for the innovation factorisation of a pair (chol_fused_pair)
+  OVP_CUDA(cudaMalloc(&c->cf_linv_s, (size_t)c->cf_maxT * 4096 * sizeof(double)));
+  OVP_CUDA(cudaMalloc(&c->cf_xch_s, ((size_t)c->cf_maxT * c->cf_maxT + 2 * c->cf_maxT) * 64 * 68 * sizeof(double)));
+  OVP_CUDA(cudaMalloc(&c->cf_diag0_s, (size_t)c->cf_maxT * 64 * sizeof(double)));
+  OVP_CUDA(cudaMalloc(&c->cf_flags_s, (size_t)(3 * c->cf_maxT + c->cf_maxT * c->cf_maxT) * sizeof(int)));
+  OVP_CUDA(cudaMemset(c->cf_linv_s, 0, (size_t)c->cf_maxT * 4096 * sizeof(double)));
+  OVP_CUDA(cudaMemset(c->cf_diag0_s, 0, (size_t)c->cf_maxT * 64 * sizeof(double)));
+  OVP_CUDA(cudaMemset(c->cf_flags_s, 0, (size_t)(3 * c->cf_maxT + c->cf_maxT * c->cf_maxT) * sizeof(int)));
   OVP_CUDA(cudaMalloc(&c->dM, (size_t)c->Nmax * c->Rcap * sizeof(double)));
   OVP_CUDA(cudaMalloc(&c->dY, (size_t)c->Nmax * c->Rcap * sizeof(double)));
   OVP_CUDA(cudaMalloc(&c->dHT, (size_t)c->Rcap * c->Rcap * sizeof(double)));
@@ -456,6 +466,10 @@ void ovp_destroy(ovp_ctx *h) {
   cudaFree(c->cf_diag0);
   cudaFree(c->cf_flags);
   cudaFree(c->cf_ctrl);
+  cudaFree(c->cf_linv_s);
+  cudaFree(c->cf_xch_s);
+  cudaFree(c->cf_diag0_s);
+  cudaFree(c->cf_flags_s);
   ws_free(c->wsG);
   ws_free(c->wsS);
   cudaFree(c->dM);

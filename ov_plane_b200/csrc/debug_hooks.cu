@@ -32,8 +32,8 @@ extern "C" int ovp_debug_chol_fused(ovp_ctx *h, int n, int mrows, int iters, dou
   const int T = (n + 63) / 64;
   const int ncta = T * (T + 1) / 2 + (mrows ? (mrows + 1 + 15) / 16 : 0);
   long long *dbg = nullptr;
-  OVP_CUDA(cudaMalloc(&dbg, ((size_t)ncta * 16 + 64) * sizeof(long long)));
-  OVP_CUDA(cudaMemset(dbg, 0, ((size_t)ncta * 16 + 64) * sizeof(long long)));
+  OVP_CUDA(cudaMalloc(&dbg, ((size_t)ncta * 16 + 128) * sizeof(long long))); // + the spine's per-step stamps, not reported here
+  OVP_CUDA(cudaMemset(dbg, 0, ((size_t)ncta * 16 + 128) * sizeof(long long)));
   float ms;
   for (int variant = 0; variant < 2; variant++) {
     for (int rep = 0; rep < 2; rep++) {
@@ -227,6 +227,117 @@ extern "C" int ovp_debug_force_dense_features(ovp_ctx *h, int on) {
 extern "C" int ovp_debug_unfused_update_products(ovp_ctx *h, int on) {
   h->c.unfused_update_products = on != 0;
   return OVP_OK;
+}
+
+// Test / A-B hook (tests/test_gpu_pipelined_factor.py): with on != 0 every later compressed update of this context factors its Gram
+// matrix and its innovation system one after the other, also when they would fit a pair (chol_fused_pair); the plan key includes
+// the setting.  Not part of the ABI in include/ovp.h.
+extern "C" int ovp_debug_sequential_factorisations(ovp_ctx *h, int on) {
+  h->c.sequential_factorisations = on != 0;
+  return OVP_OK;
+}
+
+// Test hook (tests/test_gpu_pipelined_factor.py, tools/microbench_chol.py): ovp_debug_chol_products followed by the innovation
+// factorisation of a compressed update, as gram_factor_update runs them (paired unless ovp_debug_sequential_factorisations or the pair does
+// not fit).  z = row nc of the Gram factor.  Outputs as ovp_debug_chol_products, plus LS_out (npiv x npiv: S factored in place, lower tiles
+// written, the rest left as passed in), Y_out (N x npiv), w_out (npiv), chi2_out / gate_out (gate_thresh < 0: always 1).  info[0] = 1 when
+// the pair ran.  timeline (NULL, or 64 doubles): globaltimer stamps in us relative to the first, -1 where absent:
+// [k] the Gram spine released D(k), [32 + k] the innovation spine started step k (k < 32).  Not part of the ABI in include/ovp.h.
+extern "C" int ovp_debug_chol_pair(ovp_ctx *h, const double *G, int nc, int npiv, double tol, const double *P, int N, const int *cols,
+                                   double gate_thresh, double *L_out, double *M_out, double *LS_out, double *Y_out, double *w_out,
+                                   double *chi2_out, int *gate_out, int *info, double *timeline) {
+  Ctx *c = ovp::enter(h);
+  const int n = nc + 1;
+  if (n > c->wsG.cap || npiv > c->wsS.cap || N > c->Nmax || npiv > nc || N < 1 || npiv < 1)
+    return fail(c, OVP_ERR_CAPACITY, "debug_chol_pair: too large");
+  const int ldp = (N + 1) & ~1;
+  // stamps of at most the paired grid (64 product-only CTAs is more than any launch takes) + the phase and step stamps
+  const size_t ndbg = (size_t)16 * (chol_fused_tiles(n, npiv) + chol_fused_tiles(npiv, npiv) + 64 + (N + 16) / 16) + 192;
+  char *buf = nullptr;
+  OVP_CUDA(cudaMalloc(&buf, 2 * sizeof(double) + (size_t)ldp * N * sizeof(double) + ndbg * sizeof(long long) + (size_t)nc * sizeof(int)));
+  double *dchi2 = (double *)buf;
+  int *dgate = (int *)(dchi2 + 1);
+  double *dP = dchi2 + 2;
+  long long *dbg = (long long *)(dP + (size_t)ldp * N);
+  int *dcols = (int *)(dbg + ndbg);
+  auto run = [&]() -> int {
+    const int ldg = c->wsG.cap, lds = c->wsS.cap;
+    OVP_CUDA(cudaMemsetAsync(dbg, 0, ndbg * sizeof(long long), c->stream));
+    OVP_CUDA(cudaMemsetAsync(c->wsG.S, 0, (size_t)ldg * ldg * sizeof(double), c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(c->wsG.S, (size_t)ldg * sizeof(double), G, (size_t)n * sizeof(double), (size_t)n * sizeof(double), n,
+                               cudaMemcpyHostToDevice, c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(dP, (size_t)ldp * sizeof(double), P, (size_t)N * sizeof(double), (size_t)N * sizeof(double), N,
+                               cudaMemcpyHostToDevice, c->stream));
+    OVP_CUDA(cudaMemcpyAsync(dcols, cols, (size_t)nc * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(c->wsS.S, (size_t)lds * sizeof(double), LS_out, (size_t)npiv * sizeof(double), (size_t)npiv * sizeof(double),
+                               npiv, cudaMemcpyHostToDevice, c->stream));
+    const CholProducts pr{dP, dcols, c->dM, c->wsS.S, ldp, N, nc, c->Nmax, lds};
+    const double *z = c->wsG.S + nc;
+    bool paired = false;
+    int s = chol_fused_pair(c, c->wsG.S, ldg, n, npiv, tol, pr, z, ldg, c->dY, c->Nmax, c->dvec, gate_thresh, dchi2, dgate, dbg, &paired);
+    if (!s && !paired) {
+      s = chol_fused(c, c->wsG.S, ldg, n, npiv, tol, nullptr, 0, 0, nullptr, 1, nullptr, 0, nullptr, -1.0, nullptr, nullptr, nullptr, &pr);
+      if (!s)
+        s = chol_fused(c, c->wsS.S, lds, npiv, npiv, 0.0, c->dM, c->Nmax, N, z, ldg, c->dY, c->Nmax, c->dvec, gate_thresh, dchi2, dgate);
+    }
+    if (s)
+      return s;
+    OVP_CUDA(cudaGetLastError());
+    OVP_CUDA(cudaMemcpy2DAsync(L_out, (size_t)n * sizeof(double), c->wsG.S, (size_t)ldg * sizeof(double), (size_t)n * sizeof(double), npiv,
+                               cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(M_out, (size_t)N * sizeof(double), c->dM, (size_t)c->Nmax * sizeof(double), (size_t)N * sizeof(double), npiv,
+                               cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(LS_out, (size_t)npiv * sizeof(double), c->wsS.S, (size_t)lds * sizeof(double), (size_t)npiv * sizeof(double),
+                               npiv, cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaMemcpy2DAsync(Y_out, (size_t)N * sizeof(double), c->dY, (size_t)c->Nmax * sizeof(double), (size_t)N * sizeof(double), npiv,
+                               cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaMemcpyAsync(w_out, c->dvec, (size_t)npiv * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    double chi2 = 0.0;
+    int gate = 0;
+    OVP_CUDA(cudaMemcpyAsync(&chi2, dchi2, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaMemcpyAsync(&gate, dgate, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    std::vector<long long> ts(ndbg);
+    OVP_CUDA(cudaMemcpyAsync(ts.data(), dbg, ndbg * sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
+    OVP_CUDA(cudaStreamSynchronize(c->stream));
+    if (chi2_out)
+      *chi2_out = chi2;
+    if (gate_out)
+      *gate_out = gate;
+    info[0] = paired ? 1 : 0;
+    if (timeline) { // the pair's cooperative grid: its step stamps sit after 16 per CTA and 64 phase stamps (cholfused.cu, CF_STEP_TS)
+      for (int k = 0; k < 64; k++)
+        timeline[k] = -1.0;
+      if (paired) {
+        size_t grid = 0;
+        while (grid * 16 + 192 <= ndbg && ts[grid * 16 + 15] != 0)
+          grid++; // every CTA stamps its end (slot 15)
+        const long long *st = ts.data() + grid * 16 + 64;
+        long long t0 = LLONG_MAX;
+        for (int k = 0; k < 32; k++) {
+          if (st[32 + k])
+            t0 = std::min(t0, st[32 + k]);
+          if (st[64 + k])
+            t0 = std::min(t0, st[64 + k]);
+        }
+        for (int k = 0; k < 32; k++) {
+          timeline[k] = st[32 + k] ? 1e-3 * (double)(st[32 + k] - t0) : -1.0;
+          timeline[32 + k] = st[64 + k] ? 1e-3 * (double)(st[64 + k] - t0) : -1.0;
+        }
+      }
+    }
+    return OVP_OK;
+  };
+  int st = run();
+  cudaFree(buf);
+  if (!st) {
+    int pd = 0;
+    OVP_CUDA(cudaMemcpy(&pd, c->dflags + 1, sizeof(int), cudaMemcpyDeviceToHost));
+    if (pd) {
+      cudaMemset(c->dflags + 1, 0, sizeof(int));
+      return fail(c, OVP_ERR_NOT_POSITIVE_DEFINITE, "debug_chol_pair: innovation system not positive definite");
+    }
+  }
+  return st;
 }
 
 // Test hook (tests/test_gpu_fused_products.py): one factorisation launch that also forms the update products.  G: (nc + 1) x (nc + 1)

@@ -311,9 +311,17 @@ __global__ void any_accepted_kernel(int *flag, const int *feat_flag, int n, unsi
     *flag = 0;
 }
 
+// where an update leaves w = L^-1 z, chi2 and its gate flag
+static void update_outputs(Ctx *c, double *d_chi2, int *d_gate_flag, double **w, double **chi2, int **flag) {
+  *w = c->dvec; // [0, Rcap)
+  *chi2 = d_chi2 ? d_chi2 : c->dscal;
+  *flag = d_gate_flag ? d_gate_flag : (c->dflags + 2);
+}
+
 int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const double *d_z, const double *d_Rdiag, double gate_thresh,
-                    int *d_gate_flag, double *d_chi2, bool apply, int zstride, bool defer_join, bool ht_lower, bool products_done,
+                    int *d_gate_flag, double *d_chi2, bool apply, int zstride, bool defer_join, bool ht_lower, int done,
                     const int *feat_flag, int nfeat, unsigned accept_mask) {
+  const bool products_done = done >= 1;
   if (rr <= 0 || nc <= 0)
     return OVP_OK;
   {
@@ -346,11 +354,11 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
     p.ktri = ht_lower ? 2 : 0; // row i of H = L^T is zero left of column i
     launch_gemm1(c, p);
   }
-  double *d_w = c->dvec; // [0, Rcap)
-  double *chi2 = d_chi2 ? d_chi2 : c->dscal;
-  int *flag = d_gate_flag ? d_gate_flag : (c->dflags + 2);
+  double *d_w, *chi2;
+  int *flag;
+  update_outputs(c, d_chi2, d_gate_flag, &d_w, &chi2, &flag);
   // 3-5. S = L L^T, Y = M L^-T, w = L^-1 z, chi2 = |w|^2 and the gate flag in one launch (cholfused.cu)
-  {
+  if (done < 2) {
     int st = chol_fused(c, c->wsS.S, c->wsS.cap, rr, rr, 0.0, c->dM, c->Nmax, N, d_z, zstride, c->dY, c->Nmax, d_w, gate_thresh, chi2, flag);
     if (st)
       return st;
@@ -402,7 +410,7 @@ int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, 
   const int nc1 = nc + 1;
   const MatView L = mv(c->wsG.S, c->wsG.cap);
   const double *z = c->wsG.S + nc; // row nc of the factor, read in place (stride wsG.cap)
-  bool fused = !c->unfused_update_products && c->N > 0;
+  bool fused = !c->unfused_update_products && c->N > 0, paired = false;
   if (fused) {
     if (npiv > c->wsS.cap || nc > c->Rcap)
       return fail(c, OVP_ERR_CAPACITY, "ekf_update: system %d x %d exceeds capacity %d", npiv, nc, c->Rcap);
@@ -410,7 +418,15 @@ int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, 
     if (st)
       return st;
     const CholProducts pr{c->dP, d_cols, c->dM, c->wsS.S, c->ldP, c->N, nc, c->Nmax, c->wsS.cap};
-    st = chol_fused(c, c->wsG.S, c->wsG.cap, nc1, npiv, tol, nullptr, 0, 0, nullptr, 1, nullptr, 0, nullptr, -1.0, nullptr, nullptr, nullptr, &pr);
+    // both factorisations overlapped (chol_fused_pair) when they fit co-resident together, the innovation system's as ekf_update_core
+    // launches it
+    double *d_w, *chi2;
+    int *flag;
+    update_outputs(c, d_chi2, d_gate_flag, &d_w, &chi2, &flag);
+    st = chol_fused_pair(c, c->wsG.S, c->wsG.cap, nc1, npiv, tol, pr, z, c->wsG.cap, c->dY, c->Nmax, d_w, gate_thresh, chi2, flag, nullptr,
+                         &paired);
+    if (!st && !paired)
+      st = chol_fused(c, c->wsG.S, c->wsG.cap, nc1, npiv, tol, nullptr, 0, 0, nullptr, 1, nullptr, 0, nullptr, -1.0, nullptr, nullptr, nullptr, &pr);
     if (st)
       return st;
   } else {
@@ -418,8 +434,8 @@ int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, 
     if (st)
       return st;
   }
-  return ekf_update_core(c, d_cols, nc, L, npiv, z, nullptr, gate_thresh, d_gate_flag, d_chi2, true, c->wsG.cap, defer_join, true, fused,
-                         feat_flag, nfeat, accept_mask);
+  return ekf_update_core(c, d_cols, nc, L, npiv, z, nullptr, gate_thresh, d_gate_flag, d_chi2, true, c->wsG.cap, defer_join, true,
+                         paired ? 2 : fused ? 1 : 0, feat_flag, nfeat, accept_mask);
 }
 
 } // namespace ovp

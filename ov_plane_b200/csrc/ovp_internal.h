@@ -54,6 +54,7 @@ struct Ctx {
   double gram_tol = 1e-11;   // zero-pivot rule of the Gram Cholesky, relative to the column's original diagonal (ovp_set_rank_tolerance)
   bool force_dense_features = false; // MSCKF batches take the one-block-per-feature kernel and the dense stack (ovp_debug_force_dense_features)
   bool unfused_update_products = false; // compressed updates form M and S with two GEMM launches (ovp_debug_unfused_update_products)
+  bool sequential_factorisations = false; // compressed updates never pair their two factorisations (ovp_debug_sequential_factorisations)
 #ifdef OVP_DEBUG
   // ovp_debug_msckf_gram: the feature kernels write their raw blocks to dbg_raw (when set), and with dbg_gram_stop the MSCKF launch
   // returns right after the first Gram matrix it forms, recording that plan's index in dbg_gram_plan
@@ -108,6 +109,8 @@ struct Ctx {
   // fused Cholesky (cholfused.cu): diagonal-block inverses, inter-CTA flags, epoch word
   double *cf_linv = nullptr, *cf_diag0 = nullptr, *cf_xch = nullptr;
   int *cf_flags = nullptr, *cf_ctrl = nullptr;
+  double *cf_linv_s = nullptr, *cf_diag0_s = nullptr, *cf_xch_s = nullptr; // the innovation factorisation's set in a pair
+  int *cf_flags_s = nullptr;
   int cf_maxT = 0;
   bool cf_attr_set = false;   // per context (= per device): >48 KB dynamic shared memory opt-in of chol_fused_kernel / feature kernels
   int cf_max_coresident = 0;  // co-resident CTA capacity of this device for chol_fused_kernel
@@ -199,6 +202,13 @@ int chol_fused(Ctx *c, double *A, int ld, int n, int npiv, double tol, const dou
 // every tile CTA of one chol_fused launch must be co-resident: the tile CTAs a factorisation of the leading npiv columns of an n x n
 // system needs, how many the device holds, and the widest full factorisation (a multiple of 64) that fits
 int chol_fused_tiles(int n, int npiv);
+// The two factorisations of a compressed update overlapped when they fit co-resident together: the Gram matrix A (n x n, leading npiv
+// columns) with the products `prod` and S = prod.S (npiv x npiv) in one cooperative launch, S's tiles starting as their products are
+// stored, then Y = prod.M L_S^-T, w = L_S^-1 z, chi2 and the gate (M rows: prod.N) in a launch that starts while the first runs.  Two
+// launches, bit for bit what chol_fused produces for the two one after the other.  *paired = false: nothing was launched (the pair does
+// not fit, or c->sequential_factorisations), the caller runs the two factorisations.
+int chol_fused_pair(Ctx *c, double *A, int ld, int n, int npiv, double tol, const CholProducts &prod, const double *z, int zstride, double *Y,
+                    int ldy, double *w, double gate_thresh, double *chi2, int *gate_flag, long long *dbg, bool *paired);
 int chol_fused_capacity(Ctx *c, int *max_tiles);
 int chol_fused_width(Ctx *c, int *width);
 // tile = 0: 64-wide tiles when the batch has at least one 64-tile per SM, else 32-wide; 32 / 64 force the width (test hook).
@@ -220,7 +230,8 @@ void launch_fill(Ctx *c, double *p, size_t n, double v);
 // nc state indices).  z: rr.  Rdiag: rr or nullptr (identity).  If gate_thresh >= 0, chi2 = z^T S^-1 z is compared with
 // it on the device and the update is skipped when larger (flag written to d_gate_flag, chi2 to d_chi2).  ht_lower: HT(k, j) == 0 for k < j
 // (HT is the lower Cholesky factor of the compression) - the two products skip the structural zeros.
-// products_done: M = P[:, cols] HT (in dM) and S = HT^T M[cols, :] + R (in wsS) are already formed; steps 1-2 are skipped.
+// done: 1 - M = P[:, cols] HT (in dM) and S = HT^T M[cols, :] + R (in wsS) are already formed, steps 1-2 are skipped; 2 - S is also
+// factored and Y, w, chi2 and the gate flag are formed (chol_fused_pair), steps 1-5 are skipped.
 // feat_flag (nfeat status words, or nullptr): the update is also skipped on the device when none of them is in the accepted set
 // accept_mask (bit s set: status s accepted).  A point update none of whose features passed its gate (status 1) leaves the state
 // untouched (UpdaterMSCKF.cpp:796-807), and so does a SLAM update none of whose landmarks has status 1 or 3 (UpdaterSLAM.cpp:663-664).
@@ -228,7 +239,7 @@ void launch_fill(Ctx *c, double *p, size_t n, double v);
 #define OVP_ACCEPT_SLAM ((1u << 1) | (1u << 3))
 int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const double *d_z, const double *d_Rdiag, double gate_thresh,
                     int *d_gate_flag, double *d_chi2, bool apply = true, int zstride = 1, bool defer_join = false, bool ht_lower = false,
-                    bool products_done = false, const int *feat_flag = nullptr, int nfeat = 0, unsigned accept_mask = OVP_ACCEPT_POINT);
+                    int done = 0, const int *feat_flag = nullptr, int nfeat = 0, unsigned accept_mask = OVP_ACCEPT_POINT);
 // The compressed update: factor the Gram matrix in wsG (nc + 1 columns, z last; pivots on the leading npiv) and update with H^T = L
 // (rows [0, nc)), z = row nc of the factor, R = I.  The factorisation launch also forms M and S.
 int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, double gate_thresh, int *d_gate_flag, double *d_chi2,

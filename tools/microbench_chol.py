@@ -46,3 +46,34 @@ for (nn, mm) in ((n, 0), (n, mrows), (128, 0), (64, 0)):
         print("  pivot loop of panel p starts (cycles since potrf start): " + " ".join("%d" % v for v in ls[:4]) + "  potrf entry %d, after its first barrier %d; chain warps reach the named barrier of panel 0 at %s, of panel 1 at %s" % (ls[4], ls[5], " ".join("%d" % v for v in ls[10:14]), " ".join("%d" % v for v in ls[14:18])) + "; panel 0 set-up: branch entry %d, rows loaded %d, diagonal shuffled %d" % (ls[20], ls[21], ls[22]) + "   (chain p ends at " + " ".join("%d" % ph[1 + 3 * b] for b in range(4)) + ")")
         if mm:
             print("  row-block CTAs end: min %.1f max %.1f" % (ts[T * (T + 1) // 2:, 15].min(), ts[T * (T + 1) // 2:, 15].max()))
+
+# Paired launch of a compressed update (chol_fused_pair): per step k, when the Gram spine released D(k) and when the innovation spine
+# started step k, and the lag in Gram steps.  Systems of the benchmark's shapes: a plane update (474 columns with z, 470 pivots) and the
+# point update (471, 470), 512 rows of M.
+def _p(x):
+    return x.ctypes.data_as(C.c_void_p)
+
+
+for tag, nc, npiv in (("plane", 473, 470), ("point", 470, 470)):
+    N = 512
+    rng = np.random.default_rng(nc)
+    H = rng.standard_normal((nc + 24, nc + 1))
+    G = np.asfortranarray(np.tril(H.T @ H))
+    A = rng.standard_normal((N, N))
+    P = np.asfortranarray(A @ A.T / N + np.eye(N))
+    cols = np.ascontiguousarray(np.sort(rng.choice(N, size=nc, replace=False)), dtype=np.int32)
+    L, M, Y = np.zeros((nc + 1, npiv), order="F"), np.zeros((N, npiv), order="F"), np.zeros((N, npiv), order="F")
+    LS, w, tl = np.zeros((npiv, npiv), order="F"), np.zeros(npiv), np.zeros(64)
+    chi2, gate, info = C.c_double(0.0), C.c_int(0), np.zeros(1, dtype=np.int32)
+    for _ in range(3):  # the last run's stamps
+        ctx._ck(ctx.lib.ovp_debug_chol_pair(ctx.h, _p(G), nc, npiv, C.c_double(1e-11), _p(P), N, _p(cols), C.c_double(-1.0), _p(L), _p(M), _p(LS),
+                                            _p(Y), _p(w), C.byref(chi2), C.byref(gate), _p(info), _p(tl)))
+    if not info[0]:
+        print("%s: the pair does not fit one launch on this device" % tag)
+        continue
+    Tp = (npiv + 63) // 64
+    d, s = tl[:Tp], tl[32:32 + Tp]
+    step = (d[-1] - d[0]) / max(1, Tp - 1)  # mean Gram spine step
+    print("%s update (nc=%d, npiv=%d, N=%d), pair, us from the first stamp; Gram step %.1f us" % (tag, nc, npiv, N, step))
+    for k in range(Tp):
+        print("  k=%d  Gram spine released D(k) %7.1f   innovation spine started step k %7.1f   lag %.2f Gram steps" % (k, d[k], s[k], (s[k] - d[k]) / step))
