@@ -27,8 +27,17 @@ static void ck(std::shared_ptr<State> state, int st) {
   }
 }
 
+// FeatureInitializerOptions to the library before a triangulating call: the mode (triangulate_1d / refine_features, which every updater tests
+// before it triangulates) on the context, the ten numbers returned for the call
+static ovp_triangulation_options triangulation_options(const std::shared_ptr<State> &state, const ov_core::FeatureInitializerOptions &fi) {
+  const ovp_triangulation_mode mode = {fi.triangulate_1d ? 1 : 0, fi.refine_features ? 1 : 0};
+  ck(state, ovp_set_triangulation_mode(state->ctx, &mode));
+  return {fi.max_runs, fi.init_lamda, fi.max_lamda, fi.min_dx, fi.min_dcost, fi.lam_mult, fi.min_dist, fi.max_dist, fi.max_baseline,
+          fi.max_cond_number};
+}
+
 UpdaterMSCKF::UpdaterMSCKF(UpdaterOptions &options, ov_core::FeatureInitializerOptions &feat_init_options) : _options(options) {
-  (void)feat_init_options; // the library uses the FeatureInitializerOptions defaults unless ovp_triangulation_options says otherwise
+  initializer_feat = std::shared_ptr<ov_core::FeatureInitializer>(new ov_core::FeatureInitializer(feat_init_options));
   _options.sigma_pix_sq = _options.sigma_pix * _options.sigma_pix;
 }
 
@@ -88,7 +97,8 @@ void UpdaterMSCKF::update(std::shared_ptr<State> state, std::vector<std::shared_
       fl.append(state, *f);
     std::vector<double> p(3 * vec.size());
     std::vector<int> ok(vec.size());
-    ck(state, ovp_triangulate_features(state->ctx, (int)vec.size(), fl.meas_offset.data(), fl.meas_clone.data(), fl.uvn.data(), nullptr, p.data(), ok.data()));
+    const ovp_triangulation_options tri = triangulation_options(state, initializer_feat->config());
+    ck(state, ovp_triangulate_features(state->ctx, (int)vec.size(), fl.meas_offset.data(), fl.meas_clone.data(), fl.uvn.data(), &tri, p.data(), ok.data()));
     std::vector<std::shared_ptr<ov_core::Feature>> keep;
     for (size_t i = 0; i < vec.size(); i++) {
       if (!ok[i]) {

@@ -50,6 +50,15 @@ struct Flat { // SoA view of a feature list (mono camera)
 // ---- UpdaterSLAM ----------------------------------------------------------------------------------------------------------------------
 namespace {
 // StateOptions::feat_rep_slam / feat_rep_aruco, host-only: the representation every new landmark is created in (UpdaterSLAM.cpp:231-232)
+// FeatureInitializerOptions to the library before a triangulating call: the mode (triangulate_1d / refine_features, which every updater tests
+// before it triangulates) on the context, the ten numbers returned for the call
+ovp_triangulation_options triangulation_options(const std::shared_ptr<State> &state, const ov_core::FeatureInitializerOptions &fi) {
+  const ovp_triangulation_mode mode = {fi.triangulate_1d ? 1 : 0, fi.refine_features ? 1 : 0};
+  ck(state->ctx, ovp_set_triangulation_mode(state->ctx, &mode));
+  return {fi.max_runs, fi.init_lamda, fi.max_lamda, fi.min_dx, fi.min_dcost, fi.lam_mult, fi.min_dist, fi.max_dist, fi.max_baseline,
+          fi.max_cond_number};
+}
+
 void set_landmark_options(const std::shared_ptr<State> &state) {
   const ovp_landmark_options lo = {(int)state->_options.feat_rep_slam, (int)state->_options.feat_rep_aruco};
   ck(state->ctx, ovp_set_landmark_options(state->ctx, &lo));
@@ -74,7 +83,7 @@ void refresh_landmark(const std::shared_ptr<State> &state, ov_type::Landmark &la
 
 UpdaterSLAM::UpdaterSLAM(UpdaterOptions &options_slam, UpdaterOptions &options_aruco, ov_core::FeatureInitializerOptions &feat_init_options)
     : _options_slam(options_slam), _options_aruco(options_aruco) {
-  (void)feat_init_options;
+  initializer_feat = std::shared_ptr<ov_core::FeatureInitializer>(new ov_core::FeatureInitializer(feat_init_options));
 }
 
 void UpdaterSLAM::update(std::shared_ptr<State> state, std::vector<std::shared_ptr<ov_core::Feature>> &feature_vec,
@@ -134,7 +143,8 @@ void UpdaterSLAM::delayed_init(std::shared_ptr<State> state, std::vector<std::sh
   o.chi2_multipler = _options_slam.chi2_multipler;
   o.use_plane_constraint = (state->_options.use_plane_constraint && state->_options.use_plane_constraint_slamd) ? 1 : 0;
   o.use_refine_plane_feat = state->_options.use_refine_plane_feat ? 1 : 0;
-  o.tri = nullptr; // FeatureInitializerOptions defaults
+  const ovp_triangulation_options tri = triangulation_options(state, initializer_feat->config());
+  o.tri = &tri;
   const size_t F = feature_vec.size();
   std::vector<int> feat_status(F), new_handles(F);
   std::vector<double> p_FinG(3 * F);
@@ -176,7 +186,9 @@ void UpdaterSLAM::change_anchors(std::shared_ptr<State> state) {
 }
 
 // ---- UpdaterPlane ---------------------------------------------------------------------------------------------------------------------
-UpdaterPlane::UpdaterPlane(UpdaterOptions &options, ov_core::FeatureInitializerOptions &feat_init_options) : _options(options) { (void)feat_init_options; }
+UpdaterPlane::UpdaterPlane(UpdaterOptions &options, ov_core::FeatureInitializerOptions &feat_init_options) : _options(options) {
+  initializer_feat = std::shared_ptr<ov_core::FeatureInitializer>(new ov_core::FeatureInitializer(feat_init_options));
+}
 
 void UpdaterPlane::init_vio_plane(std::shared_ptr<State> state, std::vector<std::shared_ptr<ov_core::Feature>> &feature_vec,
                                   std::vector<std::shared_ptr<ov_core::Feature>> &feature_vec_used, const std::map<size_t, size_t> &feat2plane) {
@@ -210,7 +222,8 @@ void UpdaterPlane::init_vio_plane(std::shared_ptr<State> state, std::vector<std:
   o.plane_init_min_feat = state->_options.plane_init_min_feat;
   o.plane_init_max_cond = state->_options.plane_init_max_cond;
   o.shuffle_kind = 0; // std::shuffle draws of the reference's GCC 7..10 images
-  o.tri = nullptr;    // FeatureInitializerOptions defaults
+  const ovp_triangulation_options tri = triangulation_options(state, initializer_feat->config());
+  o.tri = &tri;
   const size_t F = feature_vec.size();
   std::vector<int> feat_status(F), plane_status(F), new_handles(F);
   std::vector<double> p_FinG(3 * F), cp(3 * F);

@@ -8,5 +8,19 @@ struct UpdaterOptions {
 };
 } // namespace ov_plane
 namespace ov_core {
-struct FeatureInitializerOptions {};
+// feat/FeatureInitializerOptions.h (OpenVINS @74a63cf): its twelve fields and defaults
+struct FeatureInitializerOptions {
+  bool triangulate_1d = false;
+  bool refine_features = true;
+  int max_runs = 5;
+  double init_lamda = 1e-3;
+  double max_lamda = 1e10;
+  double min_dx = 1e-6;
+  double min_dcost = 1e-6;
+  double lam_mult = 10;
+  double min_dist = 0.10;
+  double max_dist = 60;
+  double max_baseline = 40;
+  double max_cond_number = 10000;
+};
 } // namespace ov_core

@@ -20,6 +20,7 @@ public:
                       std::vector<std::shared_ptr<ov_core::Feature>> &feature_vec_used, const std::map<size_t, size_t> &feat2plane);
 
 protected:
+  std::shared_ptr<ov_core::FeatureInitializer> initializer_feat;
   UpdaterOptions _options;
 };
 } // namespace ov_plane

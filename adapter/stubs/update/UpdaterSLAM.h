@@ -22,6 +22,7 @@ public:
   void change_anchors(std::shared_ptr<State> state);
 
 protected:
+  std::shared_ptr<ov_core::FeatureInitializer> initializer_feat;
   UpdaterOptions _options_slam;
   UpdaterOptions _options_aruco;
 };

@@ -339,9 +339,23 @@ typedef struct ovp_triangulation_options {
  * one), uv_norm = Feature::uvs_norm (undistorted normalised coordinates, 2 floats per measurement).  status[f] = 1: p_FinG[3f..]
  * is the refined position; 0: the reference would drop the feature (condition number, depth range, baseline ratio, NaN).
  * opt == NULL runs the defaults.  Tracks of any length, a clone observed twice included; malformed tracks and a null pointer are refused
- * with OVP_ERR_BAD_ARGS before anything is copied or launched. */
+ * with OVP_ERR_BAD_ARGS before anything is copied or launched.  The linear stage and whether Gauss-Newton follows are the context's
+ * triangulation mode (ovp_set_triangulation_mode): with triangulate_1d, single_triangulation_1d (rejects on depth range and NaN only) instead
+ * of single_triangulation; without refine_features, p_FinG is the linear stage's position after that stage's own rules (no baseline-ratio
+ * rule, no second depth check).  A feature that fails has status 0 and a zero position in every mode. */
 int ovp_triangulate_features(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv_norm,
                              const ovp_triangulation_options *opt, double *p_FinG, int *status);
+
+/* FeatureInitializerOptions::triangulate_1d / refine_features (feat/FeatureInitializerOptions.h), which every updater tests before it
+ * triangulates (UpdaterMSCKF.cpp:147-166, UpdaterSLAM.cpp:128-145, UpdaterPlane.cpp:139-160).  ovp_triangulate_features,
+ * ovp_plane_init_tracks and ovp_slam_delayed_init_tracks read the mode when they launch.  NULL restores ov_core's defaults {0, 1}, which
+ * behave exactly as a context that never called this.  A value other than 0 or 1 is OVP_ERR_BAD_ARGS, the mode held before is kept.
+ * Host-only: nothing is copied to the device. */
+typedef struct ovp_triangulation_mode {
+  int triangulate_1d;  /* single_triangulation_1d instead of single_triangulation */
+  int refine_features; /* single_gaussnewton after the linear stage */
+} ovp_triangulation_mode;
+int ovp_set_triangulation_mode(ovp_ctx *ctx, const ovp_triangulation_mode *m);
 
 /* ---- PlaneFitting (track_plane/PlaneFitting.cpp): plane hypothesis + refinement, the step right before the plane Jacobians ----------- */
 /* Call sites: UpdaterMSCKF.cpp:267-360, UpdaterPlane.cpp:230-267, UpdaterSLAM.cpp:171.  Both entry points take a BATCH of candidate planes
@@ -404,8 +418,9 @@ typedef struct ovp_plane_init_options {
  * (plane_init_min_feat / plane_init_max_cond) and refined jointly with the plane free (sigma_pix / fx of the current intrinsics,
  * sigma_constraint); every plane that obtained a linearisation point is then initialised like ovp_plane_init, ascending id.
  * The measurements cross to the device once; between stages only statuses, inlier flags and the refined plane come back.
- * feat_status[F]: -1 fewer than 2 measurements (erase it from feature_vec), -2 triangulation failed (keep it), 0 not a candidate,
- * 2 candidate not consumed, 1 consumed by an initialised plane (to_delete, moved to feature_vec_used).
+ * The triangulation runs in the context's mode (ovp_set_triangulation_mode): the linear stage it selects, then Gauss-Newton when
+ * refine_features.  feat_status[F]: -1 fewer than 2 measurements (erase it from feature_vec), -2 the selected triangulation stage failed
+ * (keep it), 0 not a candidate, 2 candidate not consumed, 1 consumed by an initialised plane (to_delete, moved to feature_vec_used).
  * p_FinG_out[3F]: triangulated position (for -2, whatever the failed triangulation produced, as the reference leaves it in the Feature), or
  * the refinement's output for the features that went into a refinement; zero for features with status 0 or -1.  Plane outputs, sized F entries by the caller (at most one plane per feature): *n_planes planes, every plane
  * with a candidate after triangulation, ascending id; plane_status 1 initialised, 0 rejected by initialize's chi2, -2 RANSAC returned false,
@@ -444,9 +459,11 @@ typedef struct ovp_slam_init_options {
  * had one), 3 initialised after its plane was dropped for chi2.  plane_status[F] (may be NULL): -1 not a refinement candidate, 1 refined
  * onto its plane, 0 refinement failed.  p_FinG_out[3F]: what the reference leaves in Feature::p_FinG (the refined position for a refined
  * feature, also for status 3, whose landmark holds the triangulated one; zero for -1).  new_handles[F]: the landmark's handle, or -1.
+ * The triangulation runs in the context's mode (ovp_set_triangulation_mode); -2 means that the selected stage failed.
  * Without landmark options only GLOBAL_3D landmarks are created.  With them (ovp_set_landmark_options) each landmark is created in its
  * feature's representation: 2..4 anchored in the clone of the track's last measurement with the value and first estimate set_from_xyz of
- * the triangulation's p_FinA, 1 from p_FinG, with the Jacobians of ovp_feature_jacobian_full_rep (ovp_slam_get_representation reads both).
+ * the triangulation's p_FinA (the mode's: the linear stage's p_FinA without refine_features, the refined one with it), 1 from p_FinG,
+ * with the Jacobians of ovp_feature_jacobian_full_rep (ovp_slam_get_representation reads both).
  * Refused before anything is copied or launched, with the state untouched: a null pointer, malformed tracks (the per-track rules for the
  * tracks of two or more measurements), a duplicate featid, a featid that already has a landmark (OVP_ERR_ALREADY_IN_STATE), a featid below
  * max_aruco_features while no ArUco options are set (ovp_set_aruco_options; with them tags are accepted), a feature outside GLOBAL_3D that

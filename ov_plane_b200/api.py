@@ -59,6 +59,11 @@ class FeatureTracks(C.Structure):
                 ("featid", C.c_void_p), ("planeid", C.c_void_p)]
 
 
+class TriangulationMode(C.Structure):
+    """ovp_triangulation_mode: FeatureInitializerOptions::triangulate_1d / refine_features (include/ovp.h)"""
+    _fields_ = [("triangulate_1d", C.c_int), ("refine_features", C.c_int)]
+
+
 class TriangulationOptions(C.Structure):
     """ovp_triangulation_options: ov_core's FeatureInitializerOptions (include/ovp.h)"""
     _fields_ = [("max_runs", C.c_int), ("init_lamda", C.c_double), ("max_lamda", C.c_double), ("min_dx", C.c_double), ("min_dcost", C.c_double),
@@ -594,6 +599,17 @@ class Context(object):
         tri = _tri_options(options)
         self._ck(self.lib.ovp_triangulate_features(self.h, F, _p(mo), _p(mc), _p(uvn), C.byref(tri) if tri is not None else None, _p(pf), _p(st)))
         return pf[:F], st[:F]
+
+    def set_triangulation_mode(self, triangulate_1d=False, refine_features=True):
+        """FeatureInitializerOptions::triangulate_1d / refine_features: triangulate_features, plane_init_tracks and slam_delayed_init_tracks
+        then run single_triangulation_1d instead of single_triangulation, and skip single_gaussnewton without refine_features
+        (include/ovp.h ovp_set_triangulation_mode).  triangulate_1d=None clears the mode: ov_core's defaults (False, True) again.  Each
+        switch is a bool, or 0 / 1; the library refuses any other value and keeps the mode it held."""
+        if triangulate_1d is None:
+            self._ck(self.lib.ovp_set_triangulation_mode(self.h, None))
+            return
+        m = TriangulationMode(int(triangulate_1d), int(refine_features))
+        self._ck(self.lib.ovp_set_triangulation_mode(self.h, C.byref(m)))
 
     # ---- PlaneFitting (plane hypothesis + refinement, the step before the plane Jacobians) ----
     def plane_fitting(self, feat_offset, p_FinG, min_inlier_num, max_cond, shuffle_kind=0):

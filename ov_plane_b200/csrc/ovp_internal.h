@@ -93,6 +93,9 @@ struct Ctx {
   // representation 0..4 and ovp_slam_delayed_init_tracks creates each landmark in its feature's (landmark_rep_of)
   bool has_lm_rep = false;
   ovp_landmark_options lm_rep = {0, 0};
+  // FeatureInitializerOptions::triangulate_1d / refine_features (ovp_set_triangulation_mode): the triangulation kernel every entry point
+  // launches (launch_triangulate); {0, 1} is ov_core's default
+  ovp_triangulation_mode tri_mode = {0, 1};
   std::vector<double> chi2_table;
   double *d_chi2_table = nullptr;
   int chi2_table_n = 0;

@@ -1028,8 +1028,10 @@ __global__ void cam_pose_kernel(int nh, const int *var_kind, const int *var_id, 
   for (int i = 0; i < 3; i++)
     pc[3 * (size_t)h + i] = v[4 + i] - (R[i] * cal[4] + R[3 + i] * cal[5] + R[6 + i] * cal[6]);
 }
-// FeatureInitializer::single_triangulation + single_gaussnewton on the device (triangulate_core.h), a thread per feature
+// FeatureInitializer::single_triangulation (single_triangulation_1d when OneD) + single_gaussnewton (when Refine) on the device
+// (triangulate_core.h), a thread per feature
 // p_FinA (optional): the position in the anchor camera frame as well (ovp_slam_delayed_init_tracks with anchored landmarks)
+template <bool OneD, bool Refine>
 __global__ void triangulate_kernel(int F, const int *meas_offset, const int *meas_clone, const float *uvn, const double *Rc, const double *pc,
                                    TriOptions o, double *p_FinG, int *status, double *p_FinA) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1037,7 +1039,8 @@ __global__ void triangulate_kernel(int F, const int *meas_offset, const int *mea
     return;
   const int m0 = meas_offset[f], m = meas_offset[f + 1] - m0;
   double pf[3] = {0.0, 0.0, 0.0}, pa[3] = {0.0, 0.0, 0.0};
-  const int ok = (m >= 2) ? triangulate_feature(m, meas_clone + m0, Rc, pc, uvn + 2 * (size_t)m0, o, pf, p_FinA ? pa : nullptr) : 0;
+  const int ok =
+      (m >= 2) ? triangulate_feature<OneD, Refine>(m, meas_clone + m0, Rc, pc, uvn + 2 * (size_t)m0, o, pf, p_FinA ? pa : nullptr) : 0;
   status[f] = ok;
   for (int i = 0; i < 3; i++)
     p_FinG[3 * (size_t)f + i] = pf[i];
@@ -1064,11 +1067,17 @@ static void launch_cam_poses(Ctx *c, char *d, const PoseTable &t) { // launch er
   c->launches++;
 }
 
-// F tracks (meas_offset: F + 1 entries) against the pose table t -> p_FinG (F x 3), status (F), and p_FinA (F x 3) when not null
+// F tracks (meas_offset: F + 1 entries) against the pose table t -> p_FinG (F x 3), status (F), and p_FinA (F x 3) when not null, in the
+// context's triangulation mode (ovp_set_triangulation_mode)
 static int launch_triangulate(Ctx *c, int F, const int *meas_offset, const int *meas_clone, const float *uvn, const TriOptions &o, char *d,
                               const PoseTable &t, double *p_FinG, int *status, double *p_FinA = nullptr) {
-  triangulate_kernel<<<(F + 63) / 64, 64, 0, c->stream>>>(F, meas_offset, meas_clone, uvn, (const double *)(d + t.R), (const double *)(d + t.p), o,
-                                                          p_FinG, status, p_FinA);
+  auto kernel = triangulate_kernel<false, true>;
+  if (c->tri_mode.triangulate_1d)
+    kernel = c->tri_mode.refine_features ? triangulate_kernel<true, true> : triangulate_kernel<true, false>;
+  else if (!c->tri_mode.refine_features)
+    kernel = triangulate_kernel<false, false>;
+  kernel<<<(F + 63) / 64, 64, 0, c->stream>>>(F, meas_offset, meas_clone, uvn, (const double *)(d + t.R), (const double *)(d + t.p), o, p_FinG, status,
+                                              p_FinA);
   c->launches++;
   OVP_CUDA(cudaGetLastError());
   return OVP_OK;
@@ -1203,6 +1212,20 @@ int ovp_triangulate_features(ovp_ctx *h, int F, const int *meas_offset, const in
       (st = stage_copy_out(c, p_FinG, d + b_pf, (size_t)F * 24)) || (st = stage_copy_out(c, status, d + b_st, (size_t)F * 4)))
     return st;
   OVP_CUDA(cudaStreamSynchronize(c->stream));
+  return OVP_OK;
+}
+
+int ovp_set_triangulation_mode(ovp_ctx *h, const ovp_triangulation_mode *m) {
+  using namespace ovp;
+  Ctx *c = &h->c; // host-only: launch_triangulate reads the mode when it picks the kernel
+  if (!m) {
+    c->tri_mode = {0, 1};
+    return OVP_OK;
+  }
+  if ((m->triangulate_1d != 0 && m->triangulate_1d != 1) || (m->refine_features != 0 && m->refine_features != 1))
+    return fail(c, OVP_ERR_BAD_ARGS, "set_triangulation_mode: triangulate_1d (%d) and refine_features (%d) must be 0 or 1", m->triangulate_1d,
+                m->refine_features);
+  c->tri_mode = *m;
   return OVP_OK;
 }
 

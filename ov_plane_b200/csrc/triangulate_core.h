@@ -6,6 +6,15 @@
 // max_baseline 40, max_cond_number 10000).  Camera poses: R_GtoCi = R_ItoC R_GtoIi, p_CiinG = p_IiinG - R_GtoCi^T p_IinC
 // (UpdaterMSCKF.cpp:122-140).  The anchor is the LAST measurement's camera.  Normalised coordinates are single precision and the
 // residuals are formed in single precision like ov_core (Feature::uvs_norm is an Eigen::VectorXf).
+//
+// FeatureInitializerOptions::triangulate_1d selects FeatureInitializer::single_triangulation_1d as the linear stage instead: the depth d
+// of the anchor measurement's bearing b_A = normalize([u_A, v_A, 1]) that minimises sum_k |skew(b_k) (d b_A - p_CkinA)|^2 over every
+// other measurement k (another observation from the anchor's clone included; only the anchor measurement itself is skipped), with
+// b_k = normalize(R_AtoCk^T [u_k, v_k, 1]), R_AtoCk = R_GtoCk R_GtoA^T, p_CkinA = R_GtoA (p_CkinG - p_AinG):
+//   a_k = skew(b_k) b_A,  A = sum a_k . a_k,  b = sum a_k . (skew(b_k) p_CkinA),  d = b / A,  p_FinA = d b_A.
+// It rejects when p_FinA.z < min_dist, p_FinA.z > max_dist or |p_FinA| is NaN (A = 0 gives NaN or +-inf, and one of these catches it);
+// there is no condition-number rule.  FeatureInitializerOptions::refine_features = false skips single_gaussnewton: the linear stage's
+// p_FinA, after that stage's own rules, is the result (no baseline-ratio rule, no second depth check).
 #pragma once
 #include "jacobian_core.h"
 
@@ -61,45 +70,97 @@ OVP_HD void tri_eig_minmax(const double *A, double &emin, double &emax) {
 // Camera poses come from a table indexed by idx[k] for measurement k: Rc (9 each, R_GtoCi row-major) and pc (3 each, p_CiinG);
 // uvn: 2 floats per measurement.  Returns 1 and p_FinG on success; 0 when single_triangulation or single_gaussnewton would return false.
 // p_FinA (optional): the position in the anchor camera frame, written on success (FeatureInitializer's Feature::p_FinA).
-OVP_HD int triangulate_feature(int m, const int *idx, const double *Rc, const double *pc, const float *uvn, const TriOptions &o, double *p_FinG,
-                               double *p_FinA = nullptr) {
-  const double *RA = Rc + 9 * idx[m - 1], *pA = pc + 3 * idx[m - 1]; // anchor = last measurement
-  // ---- single_triangulation ----
-  double A[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0};
-  for (int k = 0; k < m; k++) {
+// single_triangulation_1d: p_FinA (3) of the track; false when the reference would return false
+OVP_HD bool triangulate_linear_1d(int m, const int *idx, const double *Rc, const double *pc, const float *uvn, const TriOptions &o, const double *RA,
+                                  const double *pA, double *pf) {
+  double bA[3] = {(double)uvn[2 * (m - 1)], (double)uvn[2 * (m - 1) + 1], 1.0};
+  const double nA = sqrt(bA[0] * bA[0] + bA[1] * bA[1] + bA[2] * bA[2]);
+  bA[0] /= nA;
+  bA[1] /= nA;
+  bA[2] /= nA;
+  double A = 0.0, b = 0.0;
+  for (int k = 0; k < m - 1; k++) { // every measurement but the anchor's (the last)
     const double *R = Rc + 9 * idx[k], *p = pc + 3 * idx[k];
-    double RAt[9]; // R_AtoCi = R_GtoCi R_GtoA^T
+    double RAt[9]; // R_AtoCk = R_GtoCk R_GtoA^T
     for (int i = 0; i < 3; i++)
       for (int j = 0; j < 3; j++)
         RAt[3 * i + j] = R[3 * i] * RA[3 * j] + R[3 * i + 1] * RA[3 * j + 1] + R[3 * i + 2] * RA[3 * j + 2];
     double d[3] = {p[0] - pA[0], p[1] - pA[1], p[2] - pA[2]}, pCA[3];
-    mat3_vec(RA, d, pCA); // p_CiinA
+    mat3_vec(RA, d, pCA); // p_CkinA
     const double u = (double)uvn[2 * k], v = (double)uvn[2 * k + 1];
-    double bi[3] = {RAt[0] * u + RAt[3] * v + RAt[6], RAt[1] * u + RAt[4] * v + RAt[7], RAt[2] * u + RAt[5] * v + RAt[8]}; // R_AtoCi^T [u v 1]
-    const double nb = sqrt(bi[0] * bi[0] + bi[1] * bi[1] + bi[2] * bi[2]);
-    bi[0] /= nb;
-    bi[1] /= nb;
-    bi[2] /= nb;
-    // Ai = skew(b)^T skew(b) = |b|^2 I - b b^T
-    const double bb = bi[0] * bi[0] + bi[1] * bi[1] + bi[2] * bi[2];
-    double Ai[9];
-    for (int i = 0; i < 3; i++)
-      for (int j = 0; j < 3; j++)
-        Ai[3 * i + j] = ((i == j) ? bb : 0.0) - bi[i] * bi[j];
-    for (int i = 0; i < 9; i++)
-      A[i] += Ai[i];
-    for (int i = 0; i < 3; i++)
-      b[i] += Ai[3 * i] * pCA[0] + Ai[3 * i + 1] * pCA[1] + Ai[3 * i + 2] * pCA[2];
+    double bk[3] = {RAt[0] * u + RAt[3] * v + RAt[6], RAt[1] * u + RAt[4] * v + RAt[7], RAt[2] * u + RAt[5] * v + RAt[8]}; // R_AtoCk^T [u v 1]
+    const double nb = sqrt(bk[0] * bk[0] + bk[1] * bk[1] + bk[2] * bk[2]);
+    bk[0] /= nb;
+    bk[1] /= nb;
+    bk[2] /= nb;
+    // skew(b_k) x = b_k x x
+    const double a[3] = {bk[1] * bA[2] - bk[2] * bA[1], bk[2] * bA[0] - bk[0] * bA[2], bk[0] * bA[1] - bk[1] * bA[0]};
+    const double w[3] = {bk[1] * pCA[2] - bk[2] * pCA[1], bk[2] * pCA[0] - bk[0] * pCA[2], bk[0] * pCA[1] - bk[1] * pCA[0]};
+    A += a[0] * a[0] + a[1] * a[1] + a[2] * a[2];
+    b += a[0] * w[0] + a[1] * w[1] + a[2] * w[2];
   }
-  double pf[3];
-  if (!tri_solve3(A, b, pf))
-    return 0;
-  double emin, emax;
-  tri_eig_minmax(A, emin, emax);
-  const double condA = emax / emin;
+  const double depth = b / A;
+  for (int i = 0; i < 3; i++)
+    pf[i] = depth * bA[i];
   const double nrm = sqrt(pf[0] * pf[0] + pf[1] * pf[1] + pf[2] * pf[2]);
-  if (!(fabs(condA) <= o.max_cond_number) || pf[2] < o.min_dist || pf[2] > o.max_dist || nrm != nrm)
-    return 0;
+  return !(pf[2] < o.min_dist || pf[2] > o.max_dist || nrm != nrm);
+}
+
+// OneD: FeatureInitializerOptions::triangulate_1d, Refine: refine_features.  <false, true> is ov_core's default.
+template <bool OneD, bool Refine>
+OVP_HD int triangulate_feature(int m, const int *idx, const double *Rc, const double *pc, const float *uvn, const TriOptions &o, double *p_FinG,
+                               double *p_FinA = nullptr) {
+  const double *RA = Rc + 9 * idx[m - 1], *pA = pc + 3 * idx[m - 1]; // anchor = last measurement
+  // ---- single_triangulation ----  (A, b, then pf: the declaration order of the 3-D-only kernel, whose SASS <false, true> keeps)
+  double A[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0};
+  if (!OneD)
+    for (int k = 0; k < m; k++) {
+      const double *R = Rc + 9 * idx[k], *p = pc + 3 * idx[k];
+      double RAt[9]; // R_AtoCi = R_GtoCi R_GtoA^T
+      for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++)
+          RAt[3 * i + j] = R[3 * i] * RA[3 * j] + R[3 * i + 1] * RA[3 * j + 1] + R[3 * i + 2] * RA[3 * j + 2];
+      double d[3] = {p[0] - pA[0], p[1] - pA[1], p[2] - pA[2]}, pCA[3];
+      mat3_vec(RA, d, pCA); // p_CiinA
+      const double u = (double)uvn[2 * k], v = (double)uvn[2 * k + 1];
+      double bi[3] = {RAt[0] * u + RAt[3] * v + RAt[6], RAt[1] * u + RAt[4] * v + RAt[7], RAt[2] * u + RAt[5] * v + RAt[8]}; // R_AtoCi^T [u v 1]
+      const double nb = sqrt(bi[0] * bi[0] + bi[1] * bi[1] + bi[2] * bi[2]);
+      bi[0] /= nb;
+      bi[1] /= nb;
+      bi[2] /= nb;
+      // Ai = skew(b)^T skew(b) = |b|^2 I - b b^T
+      const double bb = bi[0] * bi[0] + bi[1] * bi[1] + bi[2] * bi[2];
+      double Ai[9];
+      for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++)
+          Ai[3 * i + j] = ((i == j) ? bb : 0.0) - bi[i] * bi[j];
+      for (int i = 0; i < 9; i++)
+        A[i] += Ai[i];
+      for (int i = 0; i < 3; i++)
+        b[i] += Ai[3 * i] * pCA[0] + Ai[3 * i + 1] * pCA[1] + Ai[3 * i + 2] * pCA[2];
+    }
+  double pf[3];
+  if (OneD) {
+    if (!triangulate_linear_1d(m, idx, Rc, pc, uvn, o, RA, pA, pf))
+      return 0;
+  } else {
+    if (!tri_solve3(A, b, pf))
+      return 0;
+    double emin, emax;
+    tri_eig_minmax(A, emin, emax);
+    const double condA = emax / emin;
+    const double nrm = sqrt(pf[0] * pf[0] + pf[1] * pf[1] + pf[2] * pf[2]);
+    if (!(fabs(condA) <= o.max_cond_number) || pf[2] < o.min_dist || pf[2] > o.max_dist || nrm != nrm)
+      return 0;
+  }
+  if (!Refine) { // the linear stage's result, after its own rules only
+    for (int i = 0; i < 3; i++)
+      p_FinG[i] = RA[i] * pf[0] + RA[3 + i] * pf[1] + RA[6 + i] * pf[2] + pA[i];
+    if (p_FinA)
+      for (int i = 0; i < 3; i++)
+        p_FinA[i] = pf[i];
+    return 1;
+  }
   // ---- single_gaussnewton ----
   double rho = 1.0 / pf[2], alpha = pf[0] / pf[2], beta = pf[1] / pf[2];
   double lam = o.init_lamda, eps = 10000.0;
