@@ -61,7 +61,7 @@ ovp_triangulation_options triangulation_options(const std::shared_ptr<State> &st
 
 void set_landmark_options(const std::shared_ptr<State> &state) {
   const ovp_landmark_options lo = {(int)state->_options.feat_rep_slam, (int)state->_options.feat_rep_aruco};
-  ck(state->ctx, ovp_set_landmark_options(state->ctx, &lo));
+  ck(state->ctx, ovp_set_landmark_representations(state->ctx, &lo)); // 0..5, ANCHORED_INVERSE_DEPTH_SINGLE included
 }
 // Landmark::_feat_representation, _anchor_cam_id and _anchor_clone_timestamp, value and first estimate of the landmark of featid as the
 // library holds them (the anchor's timestamp is the one of the clone whose handle the library names)
@@ -74,10 +74,20 @@ void refresh_landmark(const std::shared_ptr<State> &state, ov_type::Landmark &la
   for (const auto &clone : state->_clones_IMU)
     if (anchor >= 0 && state->handle.at(clone.second.get()) == anchor)
       landmark._anchor_clone_timestamp = clone.first;
-  Eigen::MatrixXd value(3, 1), fej(3, 1);
-  ck(state->ctx, ovp_var_get(state->ctx, state->handle.at(&landmark), value.data(), fej.data()));
+  const int h = state->handle.at(&landmark), n = ovp_var_size(state->ctx, h); // 1 for the single-depth form, as Landmark::value() is
+  Eigen::MatrixXd value(n, 1), fej(n, 1);
+  ck(state->ctx, ovp_var_get(state->ctx, h, value.data(), fej.data()));
   landmark.set_value(value);
   landmark.set_fej(fej);
+  if (rep == ov_type::LandmarkRepresentation::Representation::ANCHORED_INVERSE_DEPTH_SINGLE) { // the bearings it carries: rho p_FinA
+    Eigen::Vector3d p, pf;
+    ck(state->ctx, ovp_slam_get_xyz(state->ctx, (int64_t)landmark._featid, 0, p.data()));
+    ck(state->ctx, ovp_slam_get_xyz(state->ctx, (int64_t)landmark._featid, 1, pf.data()));
+    for (int k = 0; k < 3; k++) {
+      landmark.uv_norm_zero(k) = value(0, 0) * p(k);
+      landmark.uv_norm_zero_fej(k) = fej(0, 0) * pf(k);
+    }
+  }
 }
 } // namespace
 
@@ -104,6 +114,8 @@ void UpdaterSLAM::update(std::shared_ptr<State> state, std::vector<std::shared_p
   ck(state->ctx, ovp_slam_update(state->ctx, (int)feature_vec.size(), fl.meas_offset.data(), fl.meas_clone.data(), fl.uv.data(), fl.featid.data(),
                                  fl.planeid.data(), &uo, state->_options.use_plane_constraint_slamu ? 1 : 0, st.data(), chi.data()));
   for (size_t i = 0; i < feature_vec.size(); i++) { // 0: rejected -> the landmark is flagged for marginalisation unless a tag (:596-618)
+    if (st[i] == -1)
+      continue; // a single-depth landmark with one measurement: erased from feature_vec untouched (:410-417)
     feature_vec[i]->to_delete = true;
     if (st[i] == 0 && (int)feature_vec[i]->featid >= state->_options.max_aruco_features)
       state->_features_SLAM.at(feature_vec[i]->featid)->should_marg = true;
@@ -161,7 +173,7 @@ void UpdaterSLAM::delayed_init(std::shared_ptr<State> state, std::vector<std::sh
     if (feat_status[i] <= 0)
       continue; // erased from feature_vec
     // :283-305, :352 register the landmark with its representation, anchor, value and first estimate as the library holds them
-    auto landmark = std::make_shared<ov_type::Landmark>(3);
+    auto landmark = std::make_shared<ov_type::Landmark>(ovp_var_size(state->ctx, new_handles[i])); // 1 for the single-depth form
     landmark->_featid = f->featid;
     landmark->_unique_camera_id = 0;
     state->handle[landmark.get()] = new_handles[i];

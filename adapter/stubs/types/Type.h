@@ -64,5 +64,7 @@ public:
   double _anchor_clone_timestamp = -1;
   bool should_marg = false;
   LandmarkRepresentation::Representation _feat_representation = LandmarkRepresentation::UNKNOWN;
+  Eigen::Vector3d uv_norm_zero;     // ANCHORED_INVERSE_DEPTH_SINGLE: the bearing rho p_FinA it was set from
+  Eigen::Vector3d uv_norm_zero_fej; // and its first-estimate copy
 };
 } // namespace ov_type

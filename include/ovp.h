@@ -218,14 +218,19 @@ int ovp_msckf_update_landmarks(ovp_ctx *ctx, const ovp_feature_batch *batch, con
  * removes the features of initialised planes from its MSCKF list like UpdaterPlane.cpp:459-475. */
 int ovp_plane_init(ovp_ctx *ctx, const ovp_feature_batch *batch, const ovp_updater_options *opt, int *plane_status, int *new_handles);
 
-/* ---- UpdaterSLAM (update/UpdaterSLAM.cpp) — GLOBAL_3D landmarks, and with ovp_set_landmark_options the other four
+/* ---- UpdaterSLAM (update/UpdaterSLAM.cpp) — GLOBAL_3D landmarks, and with ovp_set_landmark_representations the other five
  * representations, mono camera ---------------------------------------------------------------------------------------------------------- */
 /* UpdaterSLAM::update from "calculate the max possible measurement size" on (:389-735): per landmark feature
  * get_feature_jacobian_full with the landmark (and its in-state plane, when use_plane_constraint and
  * _features_SLAM_to_PLANE allows it) as state columns, chi2 gate against the marginal covariance, on failure WITH a plane
  * one retry without it (:547-609), then ONE EKF update with the stack of the accepted blocks (R = I).
  * planeid[f]: the feat2plane entry of the feature (0 = none).  feat_status[f]: 1 accepted (plane constraint included when the
- * feature had one), 3 accepted after dropping the plane constraint, 0 rejected (landmark flagged should_marg).
+ * feature had one), 3 accepted after dropping the plane constraint, 0 rejected (landmark flagged should_marg), -1 not updated: an
+ * ANCHORED_INVERSE_DEPTH_SINGLE landmark with one measurement, which the projection of its bearing needs two of (:410-417); feat_chi2 is NaN,
+ * nothing is launched or copied for it, the state and its flags (should_marg, _features_SLAM_to_PLANE) are unchanged, and the rest of the
+ * batch runs exactly as it would without it.  A landmark whose size does not match its representation (1 for ANCHORED_INVERSE_DEPTH_SINGLE, 3
+ * otherwise, e.g. a variable of size 1 that ovp_initialize registered as a landmark) is refused with OVP_ERR_BAD_ARGS before anything is
+ * copied or launched.
  * Every landmark has 1..29 measurements; a longer track is refused with OVP_ERR_CAPACITY before anything is launched. */
 int ovp_slam_update(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
                     const int64_t *planeid, const ovp_updater_options *opt, int use_plane_constraint, int *feat_status,
@@ -251,25 +256,39 @@ int64_t ovp_slam_plane_of(ovp_ctx *ctx, int64_t featid); /* State::_features_SLA
  * chi2_multipler <= 0: OVP_ERR_BAD_ARGS, the options held before are kept.  Host-only: nothing is copied to the device. */
 int ovp_set_aruco_options(ovp_ctx *ctx, const ovp_updater_options *aruco);
 /* StateOptions::feat_rep_slam / feat_rep_aruco (state/StateOptions.h; UpdaterSLAM.cpp:231-232), numbered as in
- * ovp_feature_jacobian_representation, 0..4.  A feature takes feat_rep_aruco when featid < max_aruco_features, feat_rep_slam otherwise.
- * Once set:
- *  - ovp_slam_update takes landmarks in any of the five representations, each with its own anchor (ovp_slam_get_representation), in one
+ * ovp_feature_jacobian_representation.  A feature takes feat_rep_aruco when featid < max_aruco_features, feat_rep_slam otherwise.
+ * Two setters take them: ovp_set_landmark_representations takes every representation, 0..5; ovp_set_landmark_options is the same setter
+ * restricted to 0..4, which it had been before the single-depth form was supported, and keeps refusing 5, so that a host built against that
+ * contract keeps getting the refusal it handles.  Once set:
+ *  - ovp_slam_update takes landmarks in any of the six representations, each with its own anchor (ovp_slam_get_representation), in one
  *    batch (:476-522, UpdaterHelper.cpp:243-303, 411-420).  A landmark outside GLOBAL_3D that would take its in-state plane
  *    (use_plane_constraint, plane in the state, _features_SLAM_to_PLANE not 0) is refused with OVP_ERR_BAD_ARGS before anything is copied or
  *    launched: the reference's plane constraint asserts GLOBAL_3D (UpdaterHelper.cpp:455-456).  The track limit of such a batch is the
  *    same 29 measurements, the anchor's 6 columns included (a longer track: OVP_ERR_CAPACITY before anything is launched).
- *  - ovp_slam_delayed_init_tracks creates each landmark in its feature's representation, anchored (2..4) in the clone of the track's last
+ *    ANCHORED_INVERSE_DEPTH_SINGLE (5) is updated as ANCHORED_MSCKF_INVERSE_DEPTH at its p_FinA with H_f's last column as its one state
+ *    column and the two bearing columns projected out: 2m - 2 rows, gated with chi2(2m - 2) (:475-479, 503-516, 558-571).
+ *  - ovp_slam_delayed_init_tracks creates each landmark in its feature's representation, anchored (2..5) in the clone of the track's last
  *    measurement (camera 0), from the triangulation's p_FinA (:230-304).  A feature outside GLOBAL_3D that would be a plane candidate is
  *    refused up front, as above.
  *  - ovp_slam_delayed_init, which takes p_FinG only, refuses a batch in which any feature takes another representation than GLOBAL_3D.
  * Options {0, 0} behave exactly as none.  NULL clears them (the default: only GLOBAL_3D landmarks are created, and ovp_slam_update refuses
- * any other).  A value outside 0..4 is OVP_ERR_BAD_ARGS, the options held before are kept; 5 (ANCHORED_INVERSE_DEPTH_SINGLE) is not
- * supported.  Host-only: nothing is copied to the device. */
+ * any other).  A value outside the setter's range is OVP_ERR_BAD_ARGS, the options held before are kept.  Host-only: nothing is copied to
+ * the device. */
 typedef struct ovp_landmark_options {
   int feat_rep_slam;
   int feat_rep_aruco;
 } ovp_landmark_options;
+int ovp_set_landmark_representations(ovp_ctx *ctx, const ovp_landmark_options *o);
 int ovp_set_landmark_options(ovp_ctx *ctx, const ovp_landmark_options *o);
+/* Landmark::get_xyz(getfej) of a landmark in the state, in any representation: p_FinG for 0 / 1, p_FinA in its anchor's camera for 2..5.
+ * A single-depth landmark's value (ovp_var_get) is [rho] alone, as Landmark::value() is; its bearing is p_FinA * rho.  getfej reads the
+ * first-estimate row (for 5: uv_norm_zero_fej / rho_fej). */
+int ovp_slam_get_xyz(ovp_ctx *ctx, int64_t featid, int getfej, double *p_F);
+/* ov_type::Landmark::get_xyz / set_from_xyz as context-free host helpers (no device work), for any representation 0..5: value holds 3
+ * doubles (0 / 2 the position, 1 / 3 [theta, phi, rho], 4 [x/z, y/z, 1/z]) or, for 5, [rho, uv_norm_zero] (4 doubles); p_F is p_FinG for 0 / 1
+ * and p_FinA for 2..5.  These are the functions the library applies to the rows of its value tables. */
+int ovp_landmark_get_xyz(int representation, const double *value, double *p_F);
+int ovp_landmark_set_from_xyz(int representation, const double *p_F, double *value);
 
 /* ---- Anchored landmark representations (UpdaterHelper.cpp:35-193, UpdaterSLAM.cpp:684-850) -------------------------------------------- */
 /* get_feature_jacobian_full (UpdaterHelper.cpp:195-449) for any ov_type::LandmarkRepresentation (numbering as in
@@ -282,12 +301,24 @@ int ovp_feature_jacobian_full_rep(ovp_ctx *ctx, int m, const int *clone_handles,
                                   double *res, int *rows_out, int *x_order, int *x_order_n);
 /* Landmark::_feat_representation / _anchor_clone_timestamp of a landmark that is in the state: declares how its 3-vector value is read
  * (0 / 2 position, 1 / 3 [theta, phi, rho], 4 [x/z, y/z, 1/z]).  ovp_slam_update takes landmarks declared otherwise once landmark options
- * are set (ovp_set_landmark_options) and refuses them before; ovp_msckf_update_landmarks takes GLOBAL_3D landmarks only. */
+ * are set (ovp_set_landmark_options) and refuses them before; ovp_msckf_update_landmarks takes GLOBAL_3D landmarks only.  The setter refuses
+ * 5: a landmark of size 3 cannot become one of size 1, and the call carries no bearing; single-depth landmarks come from
+ * ovp_slam_delayed_init_tracks, and the getter reports 5 for them. */
 int ovp_slam_set_representation(ovp_ctx *ctx, int64_t featid, int representation, int anchor_clone_handle);
 int ovp_slam_get_representation(ovp_ctx *ctx, int64_t featid, int *representation, int *anchor_clone_handle);
 /* UpdaterSLAM::perform_anchor_change (:706-850): re-express an anchored landmark in another clone's camera frame; covariance through
- * StateHelper::EKFPropagation with the anchor-change Jacobian, value and first estimate re-anchored. */
+ * StateHelper::EKFPropagation with the anchor-change Jacobian, value and first estimate re-anchored.  For ANCHORED_INVERSE_DEPTH_SINGLE the
+ * Jacobian has one row and takes H_f_new's pseudo-inverse H_f_new^T / |H_f_new|^2 (:802-824); rho and the bearing are both reset from the
+ * re-anchored point, in the value and in the first estimate. */
 int ovp_slam_perform_anchor_change(ovp_ctx *ctx, int64_t featid, int new_anchor_clone_handle);
+/* The host algebra of ovp_slam_perform_anchor_change as a context-free helper (no device work): for a landmark of anchored representation
+ * 2..5 with value / first estimate as in ovp_landmark_get_xyz, anchored in the clone [q_GtoI, p_IinG] old7 (first estimate old_fej7), moving to
+ * new7 / new_fej7 (same_anchor = 1: the same clone) with extrinsics calib7: Phi (column-major, *phi_rows = the landmark's size, 3 or 1, by
+ * *phi_cols) over [old anchor 6][extrinsics 6 when calib_pose][new anchor 6 unless same_anchor][landmark], and the new value / first estimate
+ * (set_from_xyz of the re-anchored points).  Phi holds up to 3 x 21 doubles. */
+int ovp_anchor_change_jacobian(int representation, int do_fej, int calib_pose, int same_anchor, const double *value, const double *fej,
+                               const double *old7, const double *old_fej7, const double *new7, const double *new_fej7, const double *calib7,
+                               double *Phi, int *phi_rows, int *phi_cols, double *value_new, double *fej_new);
 /* UpdaterSLAM::change_anchors (:684-704): when the clone window is over its limit, every landmark anchored in the clone about to be
  * marginalised (the oldest) moves to the clone at the state time.  *n_changed (optional): how many landmarks moved. */
 int ovp_slam_change_anchors(ovp_ctx *ctx, int *n_changed);
@@ -460,10 +491,13 @@ typedef struct ovp_slam_init_options {
  * onto its plane, 0 refinement failed.  p_FinG_out[3F]: what the reference leaves in Feature::p_FinG (the refined position for a refined
  * feature, also for status 3, whose landmark holds the triangulated one; zero for -1).  new_handles[F]: the landmark's handle, or -1.
  * The triangulation runs in the context's mode (ovp_set_triangulation_mode); -2 means that the selected stage failed.
- * Without landmark options only GLOBAL_3D landmarks are created.  With them (ovp_set_landmark_options) each landmark is created in its
- * feature's representation: 2..4 anchored in the clone of the track's last measurement with the value and first estimate set_from_xyz of
- * the triangulation's p_FinA (the mode's: the linear stage's p_FinA without refine_features, the refined one with it), 1 from p_FinG,
- * with the Jacobians of ovp_feature_jacobian_full_rep (ovp_slam_get_representation reads both).
+ * Without landmark options only GLOBAL_3D landmarks are created.  With them (ovp_set_landmark_options / ovp_set_landmark_representations)
+ * each landmark is created in its feature's representation: 2..5 anchored in the clone of the track's last measurement with the value and
+ * first estimate set_from_xyz of the triangulation's p_FinA (the mode's: the linear stage's p_FinA without refine_features, the refined one
+ * with it), 1 from p_FinG, with the Jacobians of ovp_feature_jacobian_full_rep (ovp_slam_get_representation reads both).
+ * ANCHORED_INVERSE_DEPTH_SINGLE (5) takes the Jacobians of ANCHORED_MSCKF_INVERSE_DEPTH, projects H_f's two bearing columns out of
+ * [H_x | H_rho | r] and initialises a landmark of size 1 from the remaining 2m - 2 rows, chi2 with 2m - 2 dof (UpdaterSLAM.cpp:260-283);
+ * its value is rho = 1/z and it keeps its initial bearing (ovp_slam_get_xyz).
  * Refused before anything is copied or launched, with the state untouched: a null pointer, malformed tracks (the per-track rules for the
  * tracks of two or more measurements), a duplicate featid, a featid that already has a landmark (OVP_ERR_ALREADY_IN_STATE), a featid below
  * max_aruco_features while no ArUco options are set (ovp_set_aruco_options; with them tags are accepted), a feature outside GLOBAL_3D that

@@ -531,6 +531,21 @@ class Context(object):
         lo = LandmarkOptions(int(feat_rep_slam), int(feat_rep_slam if feat_rep_aruco is None else feat_rep_aruco))
         self._ck(self.lib.ovp_set_landmark_options(self.h, C.byref(lo)))
 
+    def set_landmark_representations(self, feat_rep_slam, feat_rep_aruco=None):
+        """set_landmark_options that also takes 5, ANCHORED_INVERSE_DEPTH_SINGLE (include/ovp.h ovp_set_landmark_representations): 0..5,
+        feat_rep_aruco defaults to feat_rep_slam, feat_rep_slam=None clears them."""
+        if feat_rep_slam is None:
+            self._ck(self.lib.ovp_set_landmark_representations(self.h, None))
+            return
+        lo = LandmarkOptions(int(feat_rep_slam), int(feat_rep_slam if feat_rep_aruco is None else feat_rep_aruco))
+        self._ck(self.lib.ovp_set_landmark_representations(self.h, C.byref(lo)))
+
+    def slam_get_xyz(self, featid, fej=False):
+        """Landmark::get_xyz(fej) of the landmark of featid: p_FinG for representations 0 / 1, p_FinA for the anchored ones 2..5"""
+        p = np.zeros(3)
+        self._ck(self.lib.ovp_slam_get_xyz(self.h, C.c_int64(int(featid)), 1 if fej else 0, _p(p)))
+        return p
+
     def slam_handle(self, featid):
         return self.lib.ovp_slam_handle(self.h, C.c_int64(int(featid)))
 

@@ -1675,6 +1675,7 @@ struct DeviceTracks {
 };
 static bool is_relative(int rep);
 static bool landmark_set_from_xyz(int rep, const double *p, double *v);
+static int landmark_store_bearing(Ctx *c, int h, const double *b); // anchors.cu
 static int stage_feature_jacobian_rep(Ctx *c, int m, const int *clone_handles, const float *uv, int representation, int anchor_clone_handle,
                                       const double *p_F, const double *p_F_fej, double sigma_px, FeatureJacobianStage *jo, int *k_out,
                                       int *extra_out, const DeviceTrack *dev = nullptr); // anchors.cu
@@ -1682,8 +1683,9 @@ static int stage_feature_jacobian_rep(Ctx *c, int m, const int *clone_handles, c
 // plane constraint when the plane is in the state, StateHelper::initialize(landmark, ..., chi2_multipler); when that fails WITH a
 // plane, detach the landmark from the plane and retry from the pre-refinement position (:310-359).  An ArUco tag takes the context's
 // ArUco options on both tries (slam_options_of).  A feature whose representation (landmark_rep_of) is not GLOBAL_3D has no plane (its
-// caller refuses it otherwise) and is initialised once, with the Jacobians of stage_feature_jacobian_rep (:230-304): anchored (2..4) in the
-// clone of its last measurement, from p_FinA (its value and first estimate are set_from_xyz(p_FinA)); rep 1 from p_FinG.  Shared by
+// caller refuses it otherwise) and is initialised once, with the Jacobians of stage_feature_jacobian_rep (:230-304): anchored (2..5) in the
+// clone of its last measurement, from p_FinA (its value and first estimate are set_from_xyz(p_FinA)); rep 1 from p_FinG.  Rep 5 takes the
+// Jacobians of rep 4, projects the two bearing columns out and initialises a 1-wide landmark from the remaining 2m - 2 rows.  Shared by
 // ovp_slam_delayed_init (dev == nullptr: each attempt stages its track from meas_clone / uv; p_FinA == nullptr, GLOBAL_3D only) and
 // ovp_slam_delayed_init_tracks (uv unused).
 static int slam_delayed_init_core(Ctx *c, int F, const int *meas_offset, const int *meas_clone, const float *uv, const DeviceTracks *dev,
@@ -1712,8 +1714,9 @@ static int slam_delayed_init_core(Ctx *c, int F, const int *meas_offset, const i
       const double *pF = is_relative(rep) ? p_FinA + 3 * (size_t)f : p_FinG + 3 * (size_t)f;
       FeatureJacobianStage j;
       int k = 3, extra = 0;
-      int st = stage_feature_jacobian_rep(c, m, cl, dev ? nullptr : uv + 2 * (size_t)meas_offset[f], rep, anc, pF, pF, fo.sigma_pix, &j, &k, &extra,
-                                          dev ? &dt : nullptr);
+      // the single-depth form takes the Jacobians of ANCHORED_MSCKF_INVERSE_DEPTH (UpdaterSLAM.cpp:233-236)
+      int st = stage_feature_jacobian_rep(c, m, cl, dev ? nullptr : uv + 2 * (size_t)meas_offset[f], rep == 5 ? 4 : rep, anc, pF, pF, fo.sigma_pix,
+                                          &j, &k, &extra, dev ? &dt : nullptr);
       if (st)
         return st;
       std::vector<int> xo;
@@ -1732,17 +1735,29 @@ static int slam_delayed_init_core(Ctx *c, int F, const int *meas_offset, const i
         return fail(c, OVP_ERR_BAD_ARGS, "delayed_init: internal column mismatch %d vs %d", n, j.hxc);
       if (c->var_table_dirty && (st = upload_var_table(c)))
         return st;
-      double v[3]; // Landmark::set_from_xyz (:283-289)
+      double v[4]; // Landmark::set_from_xyz (:283-289)
       landmark_set_from_xyz(rep, pF, v);
+      double *W = j.W(c);
+      int s = 3, rows = j.rows;
+      if (rep == 5) { // H_f's last column joins the state side, its two bearing columns are projected out of [H_x | H_rho | r] (:260-283):
+        // the landmark is initialised from the last 2m - 2 rows of [H_rho | H_x | r] with s = 1, and the chi2 takes their 2m - 2 dof
+        householder_cols_kernel<<<1, 256, 0, c->stream>>>(W, j.rows, j.rows, 3 + n + 1, 2);
+        c->launches++;
+        OVP_CUDA(cudaGetLastError());
+        W += 2 * (size_t)j.rows + 2;
+        s = 1;
+        rows = j.rows - 2;
+      }
       int acc = 0, nh = -1;
-      if ((st = initialize_core(c, OVP_KIND_LANDMARK, 3, v, v, featid[f], c->dcols, n, j.W(c), j.rows, j.rows, j.rows, 1.0, fo.chi2_multipler, 1,
-                                &acc, &nh)))
+      if ((st = initialize_core(c, OVP_KIND_LANDMARK, s, v, v, featid[f], c->dcols, n, W, j.rows, rows, rows, 1.0, fo.chi2_multipler, 1, &acc, &nh)))
         return st;
       if (acc) {
         feat_status[f] = 1;
         new_handles[f] = nh;
         c->vars[nh].rep = rep;
         c->vars[nh].anchor = anc;
+        if (rep == 5 && (st = landmark_store_bearing(c, nh, v + 1))) // the bearing it was created with, value and first estimate
+          return st;
       }
       continue;
     }

@@ -162,6 +162,44 @@ __device__ double gate_chi2(const double *A, int lda, double *T, double *S, int 
   return *s_chi2;
 }
 
+// The first nref columns of A (rows x ncols, col-major, stride lda) are reduced by nref Householder reflectors, each applied to every column
+// after its own; rows [nref, rows) of the later columns are then the left-nullspace projection of [A's other columns] (UpdaterHelper.cpp:515-546,
+// 3 reflectors instead of 3*(rows-2) sequential Givens rotations).  vbuf: rows doubles, s_beta: a shared scalar; all 128 threads participate.
+__device__ __forceinline__ void householder_left(double *A, int lda, int rows, int ncols, int nref, double *vbuf, double *s_beta, int tid) {
+  for (int j = 0; j < nref; j++) {
+    if (tid < 32) {
+      double s = 0.0;
+      for (int i = j + tid; i < rows; i += 32) {
+        double v = A[(size_t)j * lda + i];
+        s += v * v;
+      }
+      s = warp_sum(s);
+      double x0 = A[(size_t)j * lda + j];
+      double nrm = sqrt(s);
+      double alpha = (x0 > 0.0) ? -nrm : nrm;
+      double v0 = x0 - alpha;
+      double vtv = s - x0 * x0 + v0 * v0;
+      for (int i = j + tid; i < rows; i += 32)
+        vbuf[i] = (i == j) ? v0 : A[(size_t)j * lda + i];
+      if (tid == 0)
+        *s_beta = (vtv > 0.0 && nrm > 0.0) ? 2.0 / vtv : 0.0;
+    }
+    __syncthreads();
+    const double beta = *s_beta;
+    for (int cidx = j + 1 + tid; cidx < ncols; cidx += 128) {
+      double *col = A + (size_t)cidx * lda;
+      double s = 0.0;
+      for (int i = j; i < rows; i++)
+        s += vbuf[i] * col[i];
+      s *= beta;
+      if (s != 0.0)
+        for (int i = j; i < rows; i++)
+          col[i] -= s * vbuf[i];
+    }
+    __syncthreads();
+  }
+}
+
 // Local column layout of the feature block A (col-major, stride lda):
 //   [0,3) H_f | [3, 3+cf) H_x = [extrinsics 6][intrinsics 8][clone_0 6]...[clone_{m-1} 6] | [3+cf, 3+cf+3) H_cp | last: res
 // TAGS (ovp_slam_update with an ArUco tag in the batch): every feature's whitening and chi2 multiplier come from a.feat_opt.  The
@@ -171,6 +209,8 @@ __device__ double gate_chi2(const double *A, int lda, double *T, double *S, int 
 // bearing rows are taken at p_FinG and chained: H_f = (w dz/dp_FinG) dpfg_dlambda, anchor clone += (w dz/dp_FinG) dpfg_danchor,
 // extrinsics += (w dz/dp_FinG) dpfg_dcalib (UpdaterHelper.cpp:281-303, 411-420).  An anchor no measurement was taken from gets a 6-column
 // block after the track's clones, so H_x = [extrinsics][intrinsics][clone_0]...[clone_{m-1}][anchor].  Such a landmark has no plane.
+// A landmark in ANCHORED_INVERSE_DEPTH_SINGLE (rep 5) is chained as rep 4 at its p_FinA; two reflectors then project H_f's bearing columns out,
+// and rows [2, 2m) of columns [2, 3 + cf) are its gated block, local column 2 being the landmark's inverse depth.
 template <bool TAGS, bool REL = false> __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
   extern __shared__ double sm[];
   const int tid = threadIdx.x;
@@ -353,47 +393,19 @@ template <bool TAGS, bool REL = false> __global__ void __launch_bounds__(128) fe
       gid[j] = (lm >= 0) ? a.var_id[lm] + j : 0;
       gid[c_cp + j] = (ph >= 0) ? a.var_id[ph] + j : 0;
     }
-    if constexpr (REL)
+    if constexpr (REL) {
       for (int j = 0; j < xa; j++)
         gid[3 + ncal + 6 * m + j] = a.var_id[anc] + j;
+      if (rep == 5) // the landmark's one column is local column 2
+        gid[2] = a.var_id[lm];
+    }
   }
   __syncthreads();
 
   int accept = 1, rb = 0, nr = rows, cb0 = 0, ncs = 3 + cf + (has_plane ? 3 : 0); // accepted sub-block: rows [rb, rb+nr), cols [cb0, cb0+ncs)
   if (a.mode != 2) {
     // ---- left-nullspace projection of H_f: 3 Householder reflectors applied to [H_f H_x H_cp res] ----
-    for (int j = 0; j < 3; j++) {
-      if (tid < 32) {
-        double s = 0.0;
-        for (int i = j + tid; i < rows; i += 32) {
-          double v = A[(size_t)j * lda + i];
-          s += v * v;
-        }
-        s = warp_sum(s);
-        double x0 = A[(size_t)j * lda + j];
-        double nrm = sqrt(s);
-        double alpha = (x0 > 0.0) ? -nrm : nrm;
-        double v0 = x0 - alpha;
-        double vtv = s - x0 * x0 + v0 * v0;
-        for (int i = j + tid; i < rows; i += 32)
-          vbuf[i] = (i == j) ? v0 : A[(size_t)j * lda + i];
-        if (tid == 0)
-          s_beta = (vtv > 0.0 && nrm > 0.0) ? 2.0 / vtv : 0.0;
-      }
-      __syncthreads();
-      const double beta = s_beta;
-      for (int cidx = j + 1 + tid; cidx < ncols; cidx += 128) {
-        double *col = A + (size_t)cidx * lda;
-        double s = 0.0;
-        for (int i = j; i < rows; i++)
-          s += vbuf[i] * col[i];
-        s *= beta;
-        if (s != 0.0)
-          for (int i = j; i < rows; i++)
-            col[i] -= s * vbuf[i];
-      }
-      __syncthreads();
-    }
+    householder_left(A, lda, rows, ncols, 3, vbuf, &s_beta, tid);
     rb = 3;
     nr = rows - 3;
     cb0 = 3;
@@ -410,7 +422,16 @@ template <bool TAGS, bool REL = false> __global__ void __launch_bounds__(128) fe
   } else {
     // ---- SLAM landmark: no nullspace; gate with the plane constraint, on failure retry without it (UpdaterSLAM.cpp:528-622) ----
     // (an ArUco tag gates both tries with its own chi2_multipler, :545-547)
-    double chi2 = gate_chi2(A, lda, T, S, a.ldt, vbuf, Pp, a.maxcols, 0, nr, 0, ncs, gid, a.P, a.ldP, c_res, tid, &s_ok, &s_chi2);
+    if constexpr (REL)
+      if (rep == 5) { // ANCHORED_INVERSE_DEPTH_SINGLE: the third column of H_f (d / d rho) is the landmark's one state column, the two
+        // bearing columns are projected out of [H_x | H_rho | r] (UpdaterSLAM.cpp:503-516); its 2m - 2 rows are gated and stacked
+        householder_left(A, lda, rows, ncols, 2, vbuf, &s_beta, tid);
+        rb = 2;
+        nr = rows - 2;
+        cb0 = 2;
+        ncs = 1 + cf;
+      }
+    double chi2 = gate_chi2(A, lda, T, S, a.ldt, vbuf, Pp, a.maxcols, rb, nr, cb0, ncs, gid, a.P, a.ldP, c_res, tid, &s_ok, &s_chi2);
     double thr = (TAGS ? a.feat_opt[2 * f + 1] : a.chi2_mult) * a.chi2_table[nr < a.chi2_n ? nr : a.chi2_n - 1];
     int st = (s_ok && !(chi2 > thr)) ? 1 : 0;
     if (!st && has_plane) {

@@ -180,10 +180,13 @@ OVP_HD void plane_row(const double *pf, const double *pf_fej, const double *cp, 
   }
 }
 
-// ---- A landmark in the state in representation rep 1..4 (ov_type::LandmarkRepresentation; rep 0 needs none of this) ----
-// ov_type::Landmark::get_xyz: 1 / 3 store [theta, phi, rho] (rho = 1 / range), 4 [x/z, y/z, 1/z], 2 the position itself
+// ---- A landmark in the state in representation rep 1..5 (ov_type::LandmarkRepresentation; rep 0 needs none of this) ----
+// ov_type::Landmark::get_xyz: 1 / 3 store [theta, phi, rho] (rho = 1 / range), 4 [x/z, y/z, 1/z], 2 the position itself, 5 rho = 1/z in
+// slot 0 and the bearing it was created with, [x/z, y/z, 1], in slots 1..3 (p = bearing / rho)
 OVP_HD void landmark_xyz(int rep, const double *v, double *p) {
-  if (rep == 4) {
+  if (rep == 5) {
+    p[0] = v[1] / v[0], p[1] = v[2] / v[0], p[2] = v[3] / v[0];
+  } else if (rep == 4) {
     p[0] = v[0] / v[2], p[1] = v[1] / v[2], p[2] = 1.0 / v[2];
   } else if (rep == 1 || rep == 3) {
     p[0] = (1.0 / v[2]) * cos(v[0]) * sin(v[1]);
@@ -203,12 +206,13 @@ OVP_HD void landmark_d_spherical(const double *p, double *D) {
     D[i] = d[i];
 }
 // The terms get_feature_jacobian_full chains onto the bearing rows of a landmark in representation rep (UpdaterHelper.cpp:35-193, 281-303,
-// 411-420), from the landmark's value lv / first estimate lf, the anchor clone's pose anc / first-estimate pose ancf (rep 2..4) and the
-// extrinsics cal (7 each, JPL quaternion then position):
-//   out[0:3]   p_FinG (rep 2..4: R_GtoI^T R_ItoC^T (p_FinA - p_IinC) + p_IinG at the anchor's current pose), out[3:6] its first estimate
-//              (the same point for rep 2..4, :301-303);
+// 411-420), from the landmark's value lv / first estimate lf, the anchor clone's pose anc / first-estimate pose ancf (rep 2..5) and the
+// extrinsics cal (7 each, JPL quaternion then position).  Rep 5 gets the terms of rep 4 at its p_FinA: the update takes its Jacobians as
+// ANCHORED_MSCKF_INVERSE_DEPTH and keeps the third column (UpdaterSLAM.cpp:475-479, 503-516):
+//   out[0:3]   p_FinG (rep 2..5: R_GtoI^T R_ItoC^T (p_FinA - p_IinC) + p_IinG at the anchor's current pose), out[3:6] its first estimate
+//              (the same point for rep 2..5, :301-303);
 //   out[6:15]  dpfg_dlambda, column-major 3 x 3;
-//   out[15:33] dpfg_danchor and out[33:51] dpfg_dcalib, column-major 3 x 6 (rep 2..4 only), taken at the first-estimate anchor when do_fej.
+//   out[15:33] dpfg_danchor and out[33:51] dpfg_dcalib, column-major 3 x 6 (rep 2..5 only), taken at the first-estimate anchor when do_fej.
 // The same algebra as ovp_feature_jacobian_representation, written for one device thread.
 OVP_HD void landmark_rep_terms(int rep, int do_fej, const double *lv, const double *lf, const double *anc, const double *ancf,
                                const double *cal, double *out) {
@@ -274,7 +278,7 @@ OVP_HD void landmark_rep_terms(int rep, int do_fej, const double *lv, const doub
   } else {
     if (rep == 3) {
       landmark_d_spherical(pA, D);
-    } else { // lambda = (x/z, y/z, 1/z)
+    } else { // lambda = (x/z, y/z, 1/z) (rep 4, and rep 5 before its bearing columns are projected out)
       const double rho = 1.0 / pA[2], al = pA[0] / pA[2], be = pA[1] / pA[2], ir = 1.0 / rho, ir2 = 1.0 / (rho * rho);
       const double d[9] = {ir, 0.0, -ir2 * al, 0.0, ir, -ir2 * be, 0.0, 0.0, -ir2};
       for (int i = 0; i < 9; i++)

@@ -1,6 +1,7 @@
 """Time ovp_slam_update with 25 landmarks (the sim config's max_slam_in_update) held as GLOBAL_3D against the same landmarks held as
-ANCHORED_MSCKF_INVERSE_DEPTH (the update then runs feature_kernel<true, true>), over an 11-clone and a 30-clone window.  Both paths start
-from the same scene and raw tracks, and the landmarks are created by ovp_slam_delayed_init_tracks under ovp_set_landmark_options(rep, rep):
+ANCHORED_MSCKF_INVERSE_DEPTH and as ANCHORED_INVERSE_DEPTH_SINGLE (both then run feature_kernel<true, true>), over an 11-clone and a 30-clone
+window.  Both paths start
+from the same scene and raw tracks, and the landmarks are created by ovp_slam_delayed_init_tracks under ovp_set_landmark_representations(rep, rep):
 each path's covariance is then the library's own for its representation (anchored in the clone of the newest measurement), so both gate
 alike and accept the same landmarks.  Each landmark is then updated with its whole track; before every timed call the covariance and every
 value are restored (outside the timed window), so every call does the same work.  Prints one JSON line per size and path with the median /
@@ -27,7 +28,7 @@ SIZES = {
     "sim_11_clones": dict(n_clones=11, n_planes=4, F=200, m_min=3, m_max=11, plane_frac=0.5, n_slam=0, dtheta=0.05),
     "sim_30_clones": dict(n_clones=30, n_planes=4, F=400, m_min=6, m_max=20, plane_frac=0.5, n_slam=0, dtheta=0.03),
 }
-REPS = {"GLOBAL_3D": 0, "ANCHORED_MSCKF_INVERSE_DEPTH": 4}
+REPS = {"GLOBAL_3D": 0, "ANCHORED_MSCKF_INVERSE_DEPTH": 4, "ANCHORED_INVERSE_DEPTH_SINGLE": 5}
 
 
 def card():
@@ -55,7 +56,7 @@ def setup(size, rep):
     full = mk(synth.load_scenario_into(ctx, S))
     n = np.diff(full["meas_offset"])
     t = _pick(full, [f for f in range(len(n)) if 2 <= n[f] <= 29][:N_SLAM])
-    ctx.set_landmark_options(rep, rep)
+    ctx.set_landmark_representations(rep, rep)
     r = ctx.slam_delayed_init_tracks(t, use_plane_constraint=False)
     b = _pick(t, [f for f in range(t["F"]) if r["new_handles"][f] >= 0])
     return ctx, b
@@ -103,7 +104,7 @@ def main():
     a = ap.parse_args()
     gpu = card()
     for size in SIZES:
-        for path in ("GLOBAL_3D", "ANCHORED_MSCKF_INVERSE_DEPTH"):
+        for path in REPS:
             out = run(size, path, a.iters)
             out["card"] = gpu
             print(json.dumps(out))
