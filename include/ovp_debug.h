@@ -51,6 +51,10 @@ int ovp_debug_unfused_update_products(ovp_ctx *ctx, int on);
 /* on != 0: every later compressed update of this context factors its Gram matrix and its innovation system one after the other, also
  * when the two fit a pair (the innovation factorisation starting while the Gram factorisation runs) */
 int ovp_debug_sequential_factorisations(ovp_ctx *ctx, int on);
+/* on == 0: every later launch of the update chain (feature kernels, Gram, Gram reduction, the update's tail) waits for the whole of the
+ * launch before it, instead of being placed while that launch runs as its programmatic dependent (the default, on != 0).  The results
+ * are the same bit for bit.  A changed setting drops the captured graph of the prepared batch. */
+int ovp_debug_programmatic_launches(ovp_ctx *ctx, int on);
 /* one factorisation of the lower triangle of G ((nc + 1) x (nc + 1), column-major) over its leading npiv columns with pivot tolerance
  * tol, forming the update products in the same launch: with L = rows [0, nc) of the factor, M = P[:, cols] L (N x npiv) and the lower
  * tiles of S = L^T M[cols, :] + I (npiv x npiv; the 64 x 64 tiles on and below the diagonal are written, S_out's other entries are kept).  P is N x N, cols holds nc indices into it.

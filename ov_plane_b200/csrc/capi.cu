@@ -307,6 +307,9 @@ int ovp_create(const ovp_state_options *opt, int device, int max_state, int max_
   OVP_CUDA(cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking));
   OVP_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
   OVP_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
+  OVP_CUDA(cudaStreamCreateWithFlags(&c->stream3, cudaStreamNonBlocking));
+  OVP_CUDA(cudaEventCreateWithFlags(&c->ev_dfork, cudaEventDisableTiming));
+  OVP_CUDA(cudaEventCreateWithFlags(&c->ev_djoin, cudaEventDisableTiming));
   for (int i = 0; i < 8; i++)
     OVP_CUDA(cudaEventCreate(&c->ev[i]));
   c->Nmax = (max_state + 63) / 64 * 64;
@@ -507,6 +510,12 @@ void ovp_destroy(ovp_ctx *h) {
     cudaEventDestroy(c->ev_fork);
   if (c->ev_join)
     cudaEventDestroy(c->ev_join);
+  if (c->stream3)
+    cudaStreamDestroy(c->stream3);
+  if (c->ev_dfork)
+    cudaEventDestroy(c->ev_dfork);
+  if (c->ev_djoin)
+    cudaEventDestroy(c->ev_djoin);
   if (c->stream)
     cudaStreamDestroy(c->stream);
   delete h;

@@ -237,6 +237,16 @@ extern "C" int ovp_debug_sequential_factorisations(ovp_ctx *h, int on) {
   return OVP_OK;
 }
 
+// Test / A-B hook (tests/test_gpu_pdl_chain.py): with on == 0 every later launch of the update chain waits for the whole of the launch
+// before it instead of starting as its programmatic dependent (chain_launch).  A changed setting drops the prepared batch's captured
+// graph, so the next launch of the same plan captures its kernels with the new setting.  Not part of the ABI in include/ovp.h.
+extern "C" int ovp_debug_programmatic_launches(ovp_ctx *h, int on) {
+  if (h->c.programmatic != (on != 0))
+    drop_prepared_graph(&h->c);
+  h->c.programmatic = on != 0;
+  return OVP_OK;
+}
+
 // Test hook (tests/test_gpu_pipelined_factor.py, tools/microbench_chol.py): ovp_debug_chol_products followed by the innovation
 // factorisation of a compressed update, as gram_factor_update runs them (paired unless ovp_debug_sequential_factorisations or the pair does
 // not fit).  z = row nc of the Gram factor.  Outputs as ovp_debug_chol_products, plus LS_out (npiv x npiv: S factored in place, lower tiles

@@ -45,6 +45,8 @@ __device__ __forceinline__ void quat_left_update(double *q, const double *dth) {
 // independent loads (all in flight at once) and a fixed summation order.
 __global__ void __launch_bounds__(256) dx_partial_kernel(const double *Y, int ldy, int N, const double *w, int rr, double *part, int ldpart,
                                                          const int *flag) {
+  chain_wait(); // the gate flag, Y and w come from the factorisation launches
+  chain_release();
   if (flag && *flag == 0)
     return;
   __shared__ double red[4][64];
@@ -80,6 +82,8 @@ __global__ void __launch_bounds__(256) dx_partial_kernel(const double *Y, int ld
 __global__ void __launch_bounds__(128) finish_update_kernel(int nh, const int *var_id, const int *var_size, const int *var_kind, double *val,
                                                             const double *part, int ldpart, const double *P, int ldP, int *neg_flag,
                                                             const int *flag) {
+  chain_wait(); // before the early exits: this kernel's completion must imply dx_partial_kernel's
+  chain_release();
   const int h = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (h >= nh)
     return;
@@ -300,6 +304,8 @@ int join_side_stream(Ctx *c) {
 // flag &= (some feat_flag[i] is in the accepted set: bit s of accept_mask for status s): one block
 __global__ void any_accepted_kernel(int *flag, const int *feat_flag, int n, unsigned accept_mask) {
   __shared__ int any;
+  chain_wait();
+  chain_release();
   if (threadIdx.x == 0)
     any = 0;
   __syncthreads();
@@ -366,8 +372,7 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
   if (!apply)
     return OVP_OK;
   if (feat_flag) {
-    any_accepted_kernel<<<1, 256, 0, c->stream>>>(flag, feat_flag, nfeat, accept_mask);
-    c->launches++;
+    OVP_CUDA(chain_launch(c, any_accepted_kernel, dim3(1), dim3(256), 0, flag, feat_flag, nfeat, accept_mask));
   }
   // 6. P -= Y Y^T (lower tiles, mirrored) and the negative-diagonal check (StateHelper.cpp:176-187)  [skipped on the device when the gate
   //    failed].  Nothing downstream needs the new P before the next update's M = P[:, ids] H^T (or a point-feature gate), so this branch
@@ -395,10 +400,10 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
   // 7. dx = Y w and the manifold update of every variable: one launch
   int nh = (int)c->vars.size();
   double *d_part = c->dvec + (size_t)8 * c->Rcap + 2 * (size_t)c->Nmax;
-  dx_partial_kernel<<<dim3((N + 63) / 64, OVP_DX_SPLIT), 256, 0, c->stream>>>(c->dY, c->Nmax, N, d_w, rr, d_part, c->Nmax, flag);
-  finish_update_kernel<<<(nh * 32 + 127) / 128, 128, 0, c->stream>>>(nh, c->d_var_id, c->d_var_size, c->d_var_kind, c->d_val, d_part, c->Nmax, nullptr,
-                                                                      c->ldP, c->dflags, flag);
-  c->launches += 2;
+  OVP_CUDA(chain_launch(c, dx_partial_kernel, dim3((N + 63) / 64, OVP_DX_SPLIT), dim3(256), 0, c->dY, c->Nmax, N, d_w, rr,
+                        d_part, c->Nmax, flag));
+  OVP_CUDA(chain_launch(c, finish_update_kernel, dim3((nh * 32 + 127) / 128), dim3(128), 0, nh, c->d_var_id, c->d_var_size,
+                        c->d_var_kind, c->d_val, d_part, c->Nmax, nullptr, c->ldP, c->dflags, flag));
   c->host_values_stale = true;
   if (!defer_join)
     return join_side_stream(c);

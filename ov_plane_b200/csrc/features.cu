@@ -213,6 +213,8 @@ __device__ __forceinline__ void householder_left(double *A, int lda, int rows, i
 // and rows [2, 2m) of columns [2, 3 + cf) are its gated block, local column 2 being the landmark's inverse depth.
 template <bool TAGS, bool REL = false> __global__ void __launch_bounds__(128) feature_kernel(FeatArgs a) {
   extern __shared__ double sm[];
+  chain_wait();
+  chain_release();
   const int tid = threadIdx.x;
   const int f = a.feat_sel[blockIdx.x];
   const int m0 = a.meas_offset[f];
@@ -476,6 +478,8 @@ template <bool TAGS, bool REL = false> __global__ void __launch_bounds__(128) fe
 // tools/lab/dmma_lab.cu); moving this kernel to m16n8k16 is open.
 #define GRAM_KS 20
 __global__ void __launch_bounds__(128) gram_kernel(const double *Hs, int ld, int rows, int nc, int kchunk, double *part, int ldp) {
+  chain_wait();
+  chain_release();
   const int tm = blockIdx.y, tn = blockIdx.x;
   if (tm < tn)
     return;
@@ -566,6 +570,8 @@ __global__ void __launch_bounds__(128) gram_kernel(const double *Hs, int ld, int
 
 // G[i,j] (lower, i >= j) = sum_z part[z][i,j] in fixed order (deterministic)
 __global__ void gram_reduce_kernel(const double *part, int ldp, int nsplit, int nc, double *G, int ldg) {
+  chain_wait();
+  chain_release();
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= nc * nc)
     return;
@@ -586,6 +592,7 @@ __global__ void gram_reduce_kernel(const double *part, int ldp, int nsplit, int 
 struct SparseD {
   int ncal, nslots, nd, nchunk;
   const double *Dcc, *Ddc, *Dddp;
+  cudaEvent_t ready; // recorded after the D part's launch on another stream (nullptr: launched on c->stream before the SYRK)
 };
 // Gram + reduce of the stacked system Hs (rows x nc) into ws.S (lower).  With sp: Hs holds the 4-rows-per-feature SYRK operand Y and
 // the result is G = D - Y^T Y; work = algorithmic flops reported for the launch.
@@ -604,15 +611,16 @@ static int gram_of_stacked(Ctx *c, int rows, int nc, int ldHs, const SparseD *sp
   nsplit = (rows + kchunk - 1) / kchunk;
   dim3 grid(tiles, tiles, nsplit);
   prof_begin(c, PROF_GRAM, work >= 0.0 ? work : (double)nc * nc * rows); // algorithmic flops of the symmetric product: 2 * n^2 * r / 2
-  gram_kernel<<<grid, 128, 0, c->stream>>>(c->dHs, ldHs, rows, nc, kchunk, c->dPart, ldp);
-  c->launches++;
+  OVP_CUDA(chain_launch(c, gram_kernel, grid, dim3(128), 0, c->dHs, ldHs, rows, nc, kchunk, c->dPart, ldp));
   prof_end(c);
+  const dim3 rgrid((nc * nc + 255) / 256);
+  if (sp && sp->ready)
+    OVP_CUDA(cudaStreamWaitEvent(c->stream, sp->ready, 0));
   if (sp)
-    gram_reduce_sparse_kernel<<<(nc * nc + 255) / 256, 256, 0, c->stream>>>(c->dPart, ldp, nsplit, nc, sp->ncal, sp->nslots, sp->nd, sp->Dcc, sp->Ddc,
-                                                                              sp->Dddp, sp->nchunk, c->wsG.S, c->wsG.cap);
+    OVP_CUDA(chain_launch(c, gram_reduce_sparse_kernel, rgrid, dim3(256), 0, c->dPart, ldp, nsplit, nc, sp->ncal, sp->nslots, sp->nd,
+                          sp->Dcc, sp->Ddc, sp->Dddp, sp->nchunk, c->wsG.S, c->wsG.cap));
   else
-    gram_reduce_kernel<<<(nc * nc + 255) / 256, 256, 0, c->stream>>>(c->dPart, ldp, nsplit, nc, c->wsG.S, c->wsG.cap);
-  c->launches++;
+    OVP_CUDA(chain_launch(c, gram_reduce_kernel, rgrid, dim3(256), 0, c->dPart, ldp, nsplit, nc, c->wsG.S, c->wsG.cap));
   return OVP_OK;
 }
 

@@ -6,6 +6,7 @@
 #include <deque>
 #include <map>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace ovp {
@@ -47,6 +48,10 @@ struct Ctx {
   cudaStream_t stream2 = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   bool join_pending = false;
+  // D-part stream of a block-sparse Gram matrix: gram_dpart_kernel runs here beside the SYRK of the same update (both read only the
+  // feature kernel's output, the reduction needs both); forked after the feature kernel, joined before the reduction (features_host.inc)
+  cudaStream_t stream3 = nullptr;
+  cudaEvent_t ev_dfork = nullptr, ev_djoin = nullptr;
   ovp_state_options opt;
   std::string last_error;
   int64_t launches = 0;
@@ -55,6 +60,7 @@ struct Ctx {
   bool force_dense_features = false; // MSCKF batches take the one-block-per-feature kernel and the dense stack (ovp_debug_force_dense_features)
   bool unfused_update_products = false; // compressed updates form M and S with two GEMM launches (ovp_debug_unfused_update_products)
   bool sequential_factorisations = false; // compressed updates never pair their two factorisations (ovp_debug_sequential_factorisations)
+  bool programmatic = true; // chain_launch makes each update-chain kernel a programmatic dependent (ovp_debug_programmatic_launches)
 #ifdef OVP_DEBUG
   // ovp_debug_msckf_gram: the feature kernels write their raw blocks to dbg_raw (when set), and with dbg_gram_stop the MSCKF launch
   // returns right after the first Gram matrix it forms, recording that plan's index in dbg_gram_plan
@@ -180,6 +186,7 @@ int msckf_prepare(Ctx *c, const ovp_feature_batch *b, const ovp_updater_options 
 int msckf_launch(Ctx *c);
 int msckf_finish(Ctx *c, int *feat_status, double *feat_chi2, int *plane_status, double *plane_chi2, int *hx_order, int *hx_order_n);
 void free_prepared(Ctx *c);
+void drop_prepared_graph(Ctx *c); // the prepared batch's captured graph: its next launch captures the plan again
 
 // error helpers
 int fail(Ctx *c, int status, const char *fmt, ...);
@@ -189,6 +196,33 @@ int fail(Ctx *c, int status, const char *fmt, ...);
     if (e__ != cudaSuccess)                                                                                                  \
       return fail(c, OVP_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e__));                   \
   } while (0)
+
+// ---- programmatic dependent launches of the update chain ---------------------------------------------------------
+// A kernel launched through chain_launch may be placed on the SMs while the kernel before it on the stream still runs: its launch
+// latency and CTA set-up hide behind that kernel's tail.  Every such kernel calls chain_wait() in every CTA before it touches global
+// memory, so nothing it reads or writes races with an earlier kernel, and - because every CTA waits on every path - its completion
+// still implies its predecessor's, which keeps stream order transitive for the launches after it.  chain_release() right after the
+// wait lets the next dependent be placed; it takes effect once every CTA of the grid has issued it or exited, so in a multi-wave grid
+// not before the last wave is resident.  Both are no-ops in a kernel not launched as a programmatic dependent.
+__device__ __forceinline__ void chain_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void chain_release() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+// kernel<<<grid, block, smem, c->stream>>>(args...) as a programmatic dependent of the previous kernel on c->stream (unless
+// c->programmatic is off), counted in c->launches.  Returns the launch's error.
+template <class... KArgs, class... Args>
+static inline cudaError_t chain_launch(Ctx *c, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, Args &&...args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = c->stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = c->programmatic ? 1 : 0;
+  c->launches++;
+  return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
 
 // ---- linalg.cu ---------------------------------------------------------------------------------------------------
 // The two products of a compressed update, formed inside the factorisation of its Gram matrix (cholfused.cu): with L = rows [0, nc) of
