@@ -37,8 +37,9 @@ typedef enum ovp_status {
   OVP_ERR_NOT_IN_STATE = 5,      /* StateHelper.cpp:279-283,387-391 */
   OVP_ERR_ALREADY_IN_STATE = 6,  /* StateHelper.cpp:403-407 */
   OVP_ERR_CAPACITY = 7,          /* state / measurement capacity given to ovp_create exceeded, or a dense system wider than the
-                                    device can factor in one co-resident launch (64 x T columns with T(T+1)/2 <= SMs: 960 on an
-                                    H100, DESIGN.md 4.1) */
+                                    declared update width (ovp_set_max_update_width; by default the widest system the device
+                                    factors in one co-resident launch, 64 x T columns with T(T+1)/2 <= SMs: 960 on an H100,
+                                    DESIGN.md 4.1) */
   OVP_ERR_CUDA = 8,              /* CUDA runtime failure; see ovp_last_error */
   OVP_ERR_NOT_POSITIVE_DEFINITE = 9,
   OVP_ERR_TIME = 10              /* Propagator.cpp:41-51 (same / backwards timestamp), StateHelper.cpp:591-594 */
@@ -167,7 +168,8 @@ int ovp_plane_measurement_compress_inplace(ovp_ctx *ctx, double *H_x, int cols, 
  * longer track puts the whole batch on the dense stacked one, whose per-feature system must fit the CTA's shared memory.  A longer track
  * is refused with OVP_ERR_CAPACITY before anything is launched, and the message names the limit.  Every other capacity check
  * of the update (rows, columns, factorisation width) also runs before the first launch, so a refused batch leaves the state as
- * it was. */
+ * it was.  The factorisation width is the declared update width (ovp_set_max_update_width: by default 960 compressed columns on an
+ * H100, about 157 clones). */
 typedef struct ovp_feature_batch {
   int F;                         /* number of features (feature_vec after triangulation, caller's order)               */
   const int *meas_offset;        /* F+1 prefix offsets into the measurement arrays (feature tracks, above)             */
@@ -231,7 +233,9 @@ int ovp_plane_init(ovp_ctx *ctx, const ovp_feature_batch *batch, const ovp_updat
  * batch runs exactly as it would without it.  A landmark whose size does not match its representation (1 for ANCHORED_INVERSE_DEPTH_SINGLE, 3
  * otherwise, e.g. a variable of size 1 that ovp_initialize registered as a landmark) is refused with OVP_ERR_BAD_ARGS before anything is
  * copied or launched.
- * Every landmark has 1..29 measurements; a longer track is refused with OVP_ERR_CAPACITY before anything is launched. */
+ * Every landmark has 1..29 measurements; a longer track is refused with OVP_ERR_CAPACITY before anything is launched.  So is a batch
+ * whose compressed width (3 per landmark, 6 per involved clone, plus the calibration) exceeds the declared update width
+ * (ovp_set_max_update_width: by default 960 on an H100, about 300 landmarks). */
 int ovp_slam_update(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
                     const int64_t *planeid, const ovp_updater_options *opt, int use_plane_constraint, int *feat_status,
                     double *feat_chi2);
@@ -557,6 +561,14 @@ int ovp_set_use_graphs(ovp_ctx *ctx, int on);
  * column's original diagonal entry) marks a rank-deficient (gauge) direction and is dropped.  Default 1e-11; the posterior is
  * invariant over 1e-9 .. 1e-13 on every scenario in tests/ (tests/test_gpu_numerics.py). */
 int ovp_set_rank_tolerance(ovp_ctx *ctx, double tol);
+/* Widest system (columns of a compressed update's Gram matrix, rows of an innovation system) one update may factor.  0 (the default):
+ * the co-resident width of one fused launch on this device (T(T+1)/2 <= co-resident CTAs: 960 on an H100), and wider systems are refused
+ * exactly as before.  A larger width, up to the context's column capacity (max_state rounded up to 64, plus 64), lets wider systems run:
+ * they are factored in panels (DESIGN.md 4.1).  Systems within the co-resident width run the same launches and give the same bits
+ * whatever is declared.  Out of range: OVP_ERR_BAD_ARGS, the width held before is kept.  Changing it drops a prepared batch's graph. */
+int ovp_set_max_update_width(ovp_ctx *ctx, int width);
+/* the declared width (after 0 is resolved) and the co-resident width of one fused launch on this device */
+int ovp_max_update_width(ovp_ctx *ctx, int *width, int *coresident_width);
 /* bytes this ctx copied host->device / device->host since creation: every host<->device copy the library issues for the ctx (operands,
  * results, column indices, variable tables and values, status words) is counted */
 int ovp_transfer_bytes(ovp_ctx *ctx, int64_t *h2d, int64_t *d2h);

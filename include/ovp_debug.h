@@ -29,6 +29,11 @@ int ovp_debug_chol_solve(ovp_ctx *ctx, const double *A, int n, int npiv, double 
  * (zstride = 0).  chi2_out and gate_out may be NULL. */
 int ovp_debug_chol_solve_gated(ovp_ctx *ctx, const double *A, int n, int npiv, double tol, const double *M, int mrows, const double *z,
                                int zstride, double gate_thresh, double *L_out, double *Y_out, double *w_out, double *chi2_out, int *gate_out);
+/* ovp_debug_chol_solve_gated through the panelled factorisation of systems wider than one co-resident launch (DESIGN.md 4.1), with a
+ * forced panel width (a multiple of 64 up to the co-resident width; anything else: OVP_ERR_BAD_ARGS), so that narrow systems cross panel
+ * boundaries (tests/test_gpu_wide_updates.py) */
+int ovp_debug_chol_panels(ovp_ctx *ctx, int panel, const double *A, int n, int npiv, double tol, const double *M, int mrows, const double *z,
+                          int zstride, double gate_thresh, double *L_out, double *Y_out, double *w_out, double *chi2_out, int *gate_out);
 /* one product C = alpha * A B + beta * C (+ diagonal) through the DMMA GEMM (tests/test_gpu_gemm.py).  Host matrices are column-major:
  * A is a_rows x a_cols, logical A (M x K) = A, or A^T when a_trans; B is b_rows x b_cols, logical B (K x N) = B, or B^T when b_trans.
  * akidx / bkidx (length K, or NULL) gather the contraction index of A / B.  C is ldc x N, updated in place.  diag_add (length

@@ -724,6 +724,17 @@ class Context(object):
     def set_rank_tolerance(self, tol):
         self._ck(self.lib.ovp_set_rank_tolerance(self.h, C.c_double(tol)))
 
+    def set_max_update_width(self, width):
+        """Widest system one update may factor (ovp_set_max_update_width): 0 is the co-resident width of one fused launch; wider
+        systems, up to the context's column capacity, are factored in panels."""
+        self._ck(self.lib.ovp_set_max_update_width(self.h, int(width)))
+
+    def max_update_width(self):
+        """(declared width, co-resident width of one fused launch on this device)"""
+        w, cw = C.c_int(), C.c_int()
+        self._ck(self.lib.ovp_max_update_width(self.h, C.byref(w), C.byref(cw)))
+        return w.value, cw.value
+
     def set_use_graphs(self, on):
         self._ck(self.lib.ovp_set_use_graphs(self.h, int(on)))
 

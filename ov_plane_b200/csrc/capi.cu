@@ -353,6 +353,9 @@ int ovp_create(const ovp_state_options *opt, int device, int max_state, int max_
   OVP_CUDA(cudaMemset(c->cf_linv_s, 0, (size_t)c->cf_maxT * 4096 * sizeof(double)));
   OVP_CUDA(cudaMemset(c->cf_diag0_s, 0, (size_t)c->cf_maxT * 64 * sizeof(double)));
   OVP_CUDA(cudaMemset(c->cf_flags_s, 0, (size_t)(3 * c->cf_maxT + c->cf_maxT * c->cf_maxT) * sizeof(int)));
+  // systems wider than one launch (cholpanel.cu): original diagonal, z, chi2 per panel
+  OVP_CUDA(cudaMalloc(&c->cf_panel, ((size_t)2 * c->Rcap + c->cf_maxT) * sizeof(double)));
+  OVP_CUDA(cudaMemset(c->cf_panel, 0, ((size_t)2 * c->Rcap + c->cf_maxT) * sizeof(double)));
   OVP_CUDA(cudaMalloc(&c->dM, (size_t)c->Nmax * c->Rcap * sizeof(double)));
   OVP_CUDA(cudaMalloc(&c->dY, (size_t)c->Nmax * c->Rcap * sizeof(double)));
   OVP_CUDA(cudaMalloc(&c->dHT, (size_t)c->Rcap * c->Rcap * sizeof(double)));
@@ -473,6 +476,7 @@ void ovp_destroy(ovp_ctx *h) {
   cudaFree(c->cf_xch_s);
   cudaFree(c->cf_diag0_s);
   cudaFree(c->cf_flags_s);
+  cudaFree(c->cf_panel);
   ws_free(c->wsG);
   ws_free(c->wsS);
   cudaFree(c->dM);

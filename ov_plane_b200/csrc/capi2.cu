@@ -1496,6 +1496,35 @@ int ovp_set_rank_tolerance(ovp_ctx *h, double tol) {
   c->gram_tol = tol;
   return OVP_OK;
 }
+int ovp_set_max_update_width(ovp_ctx *h, int width) {
+  Ctx *c = ovp::enter(h);
+  int coresident = 0;
+  int st = chol_fused_width(c, &coresident);
+  if (st)
+    return st;
+  if (width != 0 && (width < coresident || width > c->Rcap))
+    return fail(c, OVP_ERR_BAD_ARGS, "update width %d outside [%d, %d] (0: the co-resident width)", width, coresident, c->Rcap);
+  if (width != c->max_update_width) {
+    OVP_CUDA(cudaStreamSynchronize(c->stream));
+    free_prepared(c); // a prepared batch was planned and captured under the width held before
+    c->max_update_width = width;
+  }
+  return OVP_OK;
+}
+int ovp_max_update_width(ovp_ctx *h, int *width, int *coresident_width) {
+  Ctx *c = ovp::enter(h);
+  int w = 0, cw = 0;
+  int st = update_width(c, &w);
+  if (!st)
+    st = chol_fused_width(c, &cw);
+  if (st)
+    return st;
+  if (width)
+    *width = w;
+  if (coresident_width)
+    *coresident_width = cw;
+  return OVP_OK;
+}
 int ovp_transfer_bytes(ovp_ctx *h, int64_t *h2d, int64_t *d2h) {
   *h2d = h->c.h2d_bytes;
   *d2h = h->c.d2h_bytes;

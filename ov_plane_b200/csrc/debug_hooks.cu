@@ -155,9 +155,9 @@ extern "C" int ovp_debug_gemm_split(ovp_ctx *h, int M, int N, int K, int tri, in
 // stride zstride: 1 from a vector of its own, 0 in place in a column-major workspace of leading dimension wsG.cap, the layout of the
 // compressed update (gram_factor_update reads z as the last row of the Gram factor); the rest of that workspace holds NaNs.  Not part of
 // the ABI in include/ovp.h.
-extern "C" int ovp_debug_chol_solve_gated(ovp_ctx *h, const double *A, int n, int npiv, double tol, const double *M, int mrows,
-                                          const double *z, int zstride, double gate_thresh, double *L_out, double *Y_out, double *w_out,
-                                          double *chi2_out, int *gate_out) {
+// panel = 0: one chol_fused launch; > 0: chol_panels with panels of that width
+static int debug_chol_solve(ovp_ctx *h, int panel, const double *A, int n, int npiv, double tol, const double *M, int mrows, const double *z,
+                            int zstride, double gate_thresh, double *L_out, double *Y_out, double *w_out, double *chi2_out, int *gate_out) {
   Ctx *c = ovp::enter(h);
   if (n > c->wsS.cap || mrows > c->Nmax || npiv > n || npiv > c->wsG.cap)
     return fail(c, OVP_ERR_CAPACITY, "debug_chol_solve: too large");
@@ -182,8 +182,10 @@ extern "C" int ovp_debug_chol_solve_gated(ovp_ctx *h, const double *A, int n, in
       OVP_CUDA(cudaMemcpy2DAsync(dz, (size_t)zs * sizeof(double), z, sizeof(double), sizeof(double), npiv, cudaMemcpyHostToDevice, c->stream));
     }
   }
-  int st = chol_fused(c, c->wsS.S, ld, n, npiv, tol, M ? c->dM : nullptr, c->Nmax, mrows, dz, zs, c->dY, c->Nmax, c->dvec, gate_thresh,
-                      c->dscal + 8, c->dflags + 3);
+  int st = panel ? chol_panels(c, panel, c->wsS.S, ld, n, npiv, tol, M ? c->dM : nullptr, c->Nmax, mrows, dz, zs, c->dY, c->Nmax, c->dvec,
+                               gate_thresh, c->dscal + 8, c->dflags + 3)
+                 : chol_fused(c, c->wsS.S, ld, n, npiv, tol, M ? c->dM : nullptr, c->Nmax, mrows, dz, zs, c->dY, c->Nmax, c->dvec, gate_thresh,
+                              c->dscal + 8, c->dflags + 3);
   if (st)
     return st;
   OVP_CUDA(cudaMemcpy2DAsync(L_out, (size_t)n * sizeof(double), c->wsS.S, (size_t)ld * sizeof(double), (size_t)n * sizeof(double), n,
@@ -205,6 +207,22 @@ extern "C" int ovp_debug_chol_solve_gated(ovp_ctx *h, const double *A, int n, in
     return fail(c, OVP_ERR_NOT_POSITIVE_DEFINITE, "debug_chol_solve: matrix not positive definite (strict mode)");
   }
   return OVP_OK;
+}
+extern "C" int ovp_debug_chol_solve_gated(ovp_ctx *h, const double *A, int n, int npiv, double tol, const double *M, int mrows,
+                                          const double *z, int zstride, double gate_thresh, double *L_out, double *Y_out, double *w_out,
+                                          double *chi2_out, int *gate_out) {
+  return debug_chol_solve(h, 0, A, n, npiv, tol, M, mrows, z, zstride, gate_thresh, L_out, Y_out, w_out, chi2_out, gate_out);
+}
+
+// Test hook for the panelled factorisation (tests/test_gpu_wide_updates.py): ovp_debug_chol_solve_gated through chol_panels with panels of
+// `panel` columns (a multiple of 64 up to the co-resident width), so that narrow systems cross panel boundaries.  Not part of the ABI in
+// include/ovp.h.
+extern "C" int ovp_debug_chol_panels(ovp_ctx *h, int panel, const double *A, int n, int npiv, double tol, const double *M, int mrows,
+                                     const double *z, int zstride, double gate_thresh, double *L_out, double *Y_out, double *w_out,
+                                     double *chi2_out, int *gate_out) {
+  if (panel <= 0)
+    return fail(&h->c, OVP_ERR_BAD_ARGS, "debug_chol_panels: panel width %d", panel);
+  return debug_chol_solve(h, panel, A, n, npiv, tol, M, mrows, z, zstride, gate_thresh, L_out, Y_out, w_out, chi2_out, gate_out);
 }
 
 // Test hook for the fused Cholesky (tests/test_gpu_cholfused.py, tests/test_gpu_fused_products.py): ovp_debug_chol_solve_gated with z

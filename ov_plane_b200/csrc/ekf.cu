@@ -363,9 +363,10 @@ int ekf_update_core(Ctx *c, const int *d_cols, int nc, MatView HT, int rr, const
   double *d_w, *chi2;
   int *flag;
   update_outputs(c, d_chi2, d_gate_flag, &d_w, &chi2, &flag);
-  // 3-5. S = L L^T, Y = M L^-T, w = L^-1 z, chi2 = |w|^2 and the gate flag in one launch (cholfused.cu)
+  // 3-5. S = L L^T, Y = M L^-T, w = L^-1 z, chi2 = |w|^2 and the gate flag in one launch (cholfused.cu), or in panels when S is wider
+  //      than one launch holds (cholpanel.cu)
   if (done < 2) {
-    int st = chol_fused(c, c->wsS.S, c->wsS.cap, rr, rr, 0.0, c->dM, c->Nmax, N, d_z, zstride, c->dY, c->Nmax, d_w, gate_thresh, chi2, flag);
+    int st = chol_factor(c, c->wsS.S, c->wsS.cap, rr, rr, 0.0, c->dM, c->Nmax, N, d_z, zstride, c->dY, c->Nmax, d_w, gate_thresh, chi2, flag);
     if (st)
       return st;
   }
@@ -416,6 +417,13 @@ int gram_factor_update(Ctx *c, const int *d_cols, int nc, int npiv, double tol, 
   const MatView L = mv(c->wsG.S, c->wsG.cap);
   const double *z = c->wsG.S + nc; // row nc of the factor, read in place (stride wsG.cap)
   bool fused = !c->unfused_update_products && c->N > 0, paired = false;
+  if (fused) { // a Gram matrix factored in panels forms M and S with two GEMM launches
+    bool panels = false;
+    int st = chol_needs_panels(c, nc1, npiv, &panels);
+    if (st)
+      return st;
+    fused = !panels;
+  }
   if (fused) {
     if (npiv > c->wsS.cap || nc > c->Rcap)
       return fail(c, OVP_ERR_CAPACITY, "ekf_update: system %d x %d exceeds capacity %d", npiv, nc, c->Rcap);

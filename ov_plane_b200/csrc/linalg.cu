@@ -183,9 +183,10 @@ void ws_free(DenseWs &ws) {
 }
 
 // Cholesky of the leading npiv columns of the n x n lower-stored matrix A in place (rows npiv..n-1 are solved along): one launch
-// of the fused kernel (cholfused.cu).  Pivots <= tol * original diagonal are treated as exact zeros (rank-deficient Gram matrices).
+// of the fused kernel (cholfused.cu), or its panels when the system is wider (cholpanel.cu).  Pivots <= tol * original diagonal are
+// treated as exact zeros (rank-deficient Gram matrices).
 int chol_partial(Ctx *c, double *A, int ld, int n, int npiv, double tol) {
-  return chol_fused(c, A, ld, n, npiv, tol, nullptr, 0, 0, nullptr, 1, nullptr, 0, nullptr, -1.0, nullptr, nullptr);
+  return chol_factor(c, A, ld, n, npiv, tol, nullptr, 0, 0, nullptr, 1, nullptr, 0, nullptr, -1.0, nullptr, nullptr);
 }
 
 // stand-alone Householder left-nullspace projection on a global-memory matrix (col-major, ld): reflectors from the first

@@ -123,6 +123,8 @@ struct Ctx {
   int cf_maxT = 0;
   bool cf_attr_set = false;   // per context (= per device): >48 KB dynamic shared memory opt-in of chol_fused_kernel / feature kernels
   int cf_max_coresident = 0;  // co-resident CTA capacity of this device for chol_fused_kernel
+  int max_update_width = 0;   // ovp_set_max_update_width (0: the co-resident width of one fused launch)
+  double *cf_panel = nullptr; // panelled factorisation (cholpanel.cu): original diagonal (Rcap), z (Rcap), chi2 per panel (cf_maxT)
   bool feat_smem_set = false;
   int max_meas_rows = 0;
   double *dHs = nullptr;       // stacked [H_x | H_cp | res], max_meas_rows x (Rcap) col-major
@@ -233,9 +235,16 @@ struct CholProducts {
   double *M, *S;
   int ldp, N, nc, ldm, lds;
 };
+// diag0 (optional): the reference diagonal of the zero-pivot rule for the npiv pivots, in place of the diagonal the launch loads (a panel
+// of chol_panels, whose diagonal the panels before it have downdated)
 int chol_fused(Ctx *c, double *A, int ld, int n, int npiv, double tol, const double *M, int ldm, int mrows, const double *z, int zstride,
                double *Y, int ldy, double *w, double gate_thresh, double *chi2, int *gate_flag, long long *dbg = nullptr,
-               const CholProducts *prod = nullptr);
+               const CholProducts *prod = nullptr, double *diag0 = nullptr);
+// Y = M L^-T, w = L^-1 z and chi2 = |w|^2 (no gate) against the factor the chol_fused launch before it on the stream left in the exchange
+// slots (a factorisation of the same n, npiv): the second launch of chol_fused's two-launch fallback, on a right-hand side of its own.
+// Y may be M (each row block reads its rows whole before it writes them).
+int chol_fused_rows(Ctx *c, double *A, int ld, int n, int npiv, const double *M, int ldm, int mrows, const double *z, int zstride, double *Y,
+                    int ldy, double *w, double *chi2);
 // every tile CTA of one chol_fused launch must be co-resident: the tile CTAs a factorisation of the leading npiv columns of an n x n
 // system needs, how many the device holds, and the widest full factorisation (a multiple of 64) that fits
 int chol_fused_tiles(int n, int npiv);
@@ -248,6 +257,22 @@ int chol_fused_pair(Ctx *c, double *A, int ld, int n, int npiv, double tol, cons
                     int ldy, double *w, double gate_thresh, double *chi2, int *gate_flag, long long *dbg, bool *paired);
 int chol_fused_capacity(Ctx *c, int *max_tiles);
 int chol_fused_width(Ctx *c, int *width);
+// ---- cholpanel.cu: systems wider than one co-resident launch ----
+// the widest system one update may factor (ovp_set_max_update_width; 0 declared: chol_fused_width)
+int update_width(Ctx *c, int *width);
+// *panels: the factorisation of the leading npiv columns of an n x n system runs in panels (chol_panels) - it does not fit one
+// co-resident launch and n is within the declared width
+int chol_needs_panels(Ctx *c, int n, int npiv, bool *panels);
+// The contract of chol_fused without products, for a system of any width up to the workspaces: the columns are factored in panels of
+// `width` (a multiple of 64, at most chol_fused_width), each one chol_fused launch on its diagonal block, its rows below solved against it,
+// and the trailing blocks downdated with the DMMA GEMM; chi2 and the gate flag are formed from the panels' parts at the end.  Every pivot
+// is compared with its column's original diagonal.  Y receives M's columns and is worked in place; M and z are only read.
+int chol_panels(Ctx *c, int width, double *A, int ld, int n, int npiv, double tol, const double *M, int ldm, int mrows, const double *z,
+                int zstride, double *Y, int ldy, double *w, double gate_thresh, double *chi2, int *gate_flag);
+// The one entry of every update's factorisation: chol_fused when the system fits co-resident, chol_panels (panels of chol_fused_width)
+// when it does not and the declared width allows it; otherwise chol_fused's refusal.
+int chol_factor(Ctx *c, double *A, int ld, int n, int npiv, double tol, const double *M, int ldm, int mrows, const double *z, int zstride,
+                double *Y, int ldy, double *w, double gate_thresh, double *chi2, int *gate_flag);
 // tile = 0: 64-wide tiles when the batch has at least one 64-tile per SM, else 32-wide; 32 / 64 force the width (test hook).
 // Returns the tile width launched (0: nothing to do).
 int launch_gemm(Ctx *c, const GemmBatch &b, int tile = 0);
@@ -255,7 +280,7 @@ int launch_gemm(Ctx *c, const GemmBatch &b, int tile = 0);
 int gemm_plan(const Ctx *c, const GemmBatch &b, int tile, int *nchunk, int *kc);
 void launch_gemm1(Ctx *c, const GemmProblem &p, const int *flag = nullptr);
 // In-place blocked Cholesky of the leading `npiv` pivots of the symmetric (lower-stored) matrix A (size n x n, ld):
-int chol_partial(Ctx *c, double *A, int ld, int n, int npiv, double tol); // one launch of chol_fused
+int chol_partial(Ctx *c, double *A, int ld, int n, int npiv, double tol); // chol_factor without a right-hand side
 int ws_alloc(Ctx *c, DenseWs &ws, int cap);
 void ws_free(DenseWs &ws);
 // y = alpha * A(m x k view) * x  (one warp per row)

@@ -1,6 +1,7 @@
 // Unity translation unit of libovp.so (one TU: kernels defined in one file are launched from another).
 #include "linalg.cu"
 #include "cholfused.cu"
+#include "cholpanel.cu"
 #include "ekf.cu"
 #include "features.cu"
 #include "capi.cu"
