@@ -66,6 +66,12 @@ int ovp_debug_programmatic_launches(ovp_ctx *ctx, int on);
  * L_out receives the factor's (nc + 1) x npiv columns. */
 int ovp_debug_chol_products(ovp_ctx *ctx, const double *G, int nc, int npiv, double tol, const double *P, int N, const int *cols,
                             double *L_out, double *M_out, double *S_out);
+/* width > 0: every later factorisation of this context wider than width columns runs in panels of width (width: a multiple of 64 up
+ * to the co-resident width of one fused launch; anything else: OVP_ERR_BAD_ARGS), the Gram matrix of a compressed update and its
+ * innovation system alike, so that a compressed update forms M and S with two GEMM launches as one wider than a launch does
+ * (tests/test_gpu_msckf_point_reference.py).  width = 0 (the default): off.  Whether an update is compressed is still decided on the
+ * co-resident width.  A changed setting re-plans the prepared batch and drops its captured graph. */
+int ovp_debug_update_panel_width(ovp_ctx *ctx, int width);
 /* ovp_debug_chol_products followed by the innovation factorisation of the compressed update, as the update runs them (as a pair when
  * they fit co-resident together and ovp_debug_sequential_factorisations is off, else one after the other): with z = row nc of the Gram
  * factor, S = L_S L_S^T (LS_out: S's lower tiles on input as S_out above, the factor on output), Y = M L_S^-T (Y_out, N x npiv),

@@ -52,10 +52,15 @@ int update_width(Ctx *c, int *width) {
   return chol_fused_width(c, width);
 }
 
+// A forced panel width (ovp_debug_update_panel_width) panels every system wider than it, whatever one launch would hold.
 int chol_needs_panels(Ctx *c, int n, int npiv, bool *panels) {
   *panels = false;
   if (npiv <= 0)
     return OVP_OK;
+  if (c->update_panel_width > 0) {
+    *panels = n > c->update_panel_width;
+    return OVP_OK;
+  }
   int cap = 0, width = 0;
   int st = chol_fused_capacity(c, &cap);
   if (st)
@@ -130,9 +135,8 @@ int chol_factor(Ctx *c, double *A, int ld, int n, int npiv, double tol, const do
     return st;
   if (!panels)
     return chol_fused(c, A, ld, n, npiv, tol, M, ldm, mrows, z, zstride, Y, ldy, w, gate_thresh, chi2, gate_flag);
-  int width = 0;
-  st = chol_fused_width(c, &width);
-  if (st)
+  int width = c->update_panel_width;
+  if (width <= 0 && (st = chol_fused_width(c, &width)))
     return st;
   return chol_panels(c, width, A, ld, n, npiv, tol, M, ldm, mrows, z, zstride, Y, ldy, w, gate_thresh, chi2, gate_flag);
 }

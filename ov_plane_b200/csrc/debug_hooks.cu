@@ -265,6 +265,26 @@ extern "C" int ovp_debug_programmatic_launches(ovp_ctx *h, int on) {
   return OVP_OK;
 }
 
+// Test hook (tests/test_gpu_msckf_point_reference.py): width > 0 factors every later system of this context wider than width columns
+// (a multiple of 64 up to the co-resident width) in panels of width, the Gram matrix of a compressed update and its innovation system
+// alike (chol_needs_panels, chol_factor), so that a compressed update takes the route of one wider than a launch: chol_partial in
+// panels, M and S by two GEMM launches, the innovation system in panels.  width = 0: off.  Whether an update is compressed is still
+// decided on the co-resident width.  The setting is part of the plan key; a change also drops the captured graph.  Not part of the ABI
+// in include/ovp.h.
+extern "C" int ovp_debug_update_panel_width(ovp_ctx *h, int width) {
+  Ctx *c = ovp::enter(h);
+  int cw = 0;
+  int st = chol_fused_width(c, &cw);
+  if (st)
+    return st;
+  if (width != 0 && (width < 64 || width % 64 || width > cw))
+    return fail(c, OVP_ERR_BAD_ARGS, "debug_update_panel_width: %d is not 0 or a multiple of 64 up to the co-resident width %d", width, cw);
+  if (c->update_panel_width != width)
+    drop_prepared_graph(c);
+  c->update_panel_width = width;
+  return OVP_OK;
+}
+
 // Test hook (tests/test_gpu_pipelined_factor.py, tools/microbench_chol.py): ovp_debug_chol_products followed by the innovation
 // factorisation of a compressed update, as gram_factor_update runs them (paired unless ovp_debug_sequential_factorisations or the pair does
 // not fit).  z = row nc of the Gram factor.  Outputs as ovp_debug_chol_products, plus LS_out (npiv x npiv: S factored in place, lower tiles

@@ -61,6 +61,7 @@ struct Ctx {
   bool unfused_update_products = false; // compressed updates form M and S with two GEMM launches (ovp_debug_unfused_update_products)
   bool sequential_factorisations = false; // compressed updates never pair their two factorisations (ovp_debug_sequential_factorisations)
   bool programmatic = true; // chain_launch makes each update-chain kernel a programmatic dependent (ovp_debug_programmatic_launches)
+  int update_panel_width = 0; // > 0: every factorisation wider than this runs in panels of this width (ovp_debug_update_panel_width)
 #ifdef OVP_DEBUG
   // ovp_debug_msckf_gram: the feature kernels write their raw blocks to dbg_raw (when set), and with dbg_gram_stop the MSCKF launch
   // returns right after the first Gram matrix it forms, recording that plan's index in dbg_gram_plan

@@ -95,14 +95,17 @@ def kept_system(L):
     return L[:nc, :].T.copy(), L[nc, :].copy()
 
 
-def slam_bounds(P, cols, X, G, ref, tol=GRAM_TOL):
-    """(dx bound, P+ bound Jacobi-scaled by P, factor info) of the library's update against slam_update_reference(P, cols, X): G the
-    library's Gram matrix (nc1 x nc1, lower triangle read), ref the reference.  The factor info: dict(L, zero, ratio)."""
+def gram_route_bounds(P, cols, G, ref, tol=GRAM_TOL, dG=None, kref=None):
+    """The bound terms of an update that runs on the factor of its Gram matrix G (nc1 x nc1, lower triangle read) rather than on its
+    stacked rows, against the reference ref: the factorisation's backward error 2 (n + 1) eps |L| |L^T| (n = nc + 1) plus dG (another
+    element-wise bound of G's own error, or None), tol G_jj and sqrt(tol G_jj G_kk) on every dropped pivot, carried to the posterior by
+    info_effects; and kalman_bounds of the kept system H = L^T, r = the factor's last row (kref: its kalman(), computed when None).
+    Returns (ddx, dP Jacobi-scaled by P, kept dx bound, kept P+ bound, factor info dict(L, zero, ratio))."""
     nc = len(cols)
     L, zero, ratio = ld_factor(G, nc, tol)
     aL = np.abs(np.asarray(L, dtype=np.float64))
-    dG = gram_bound(X) + 2.0 * (nc + 2) * EPS * (aL @ aL.T)
-    dK = factor_dK(L, zero, G, tol, dG=dG)
+    dGf = 2.0 * (nc + 2) * EPS * (aL @ aL.T)
+    dK = factor_dK(L, zero, G, tol, dG=dGf if dG is None else dG + dGf)
     # a dropped pivot discards its whole column of the Schur complement, not only its diagonal: |S_kj| <= sqrt(S_jj S_kk) <=
     # sqrt(tol G_jj G_kk) off the diagonal
     g = np.sqrt(np.abs(np.diag(np.asarray(G, dtype=np.float64))))
@@ -113,12 +116,21 @@ def slam_bounds(P, cols, X, G, ref, tol=GRAM_TOL):
         dK[:, j] += off
     Pp, dx = np.asarray(ref["P"], dtype=np.float64), np.asarray(ref["dx"], dtype=np.float64)
     dPi, ddx, _ = info_effects(Pp[:, list(cols)], dx[list(cols)], dK)
-    dxb, dPb, _ = kalman_bounds(P, list(cols), X[:, :nc], ref)
     Hk, rk = kept_system(L)
-    kref = kalman(P, list(cols), Hk, rk, None)
+    if kref is None:
+        kref = kalman(P, list(cols), Hk, rk, None)
     dxk, dPk, _ = kalman_bounds(P, list(cols), Hk, kref)
     sd = np.sqrt(np.diag(np.asarray(P, dtype=np.float64)))
-    return np.maximum(dxb, dxk) + ddx, np.maximum(dPb, dPk) + dPi / np.outer(sd, sd), dict(L=L, zero=zero, ratio=ratio)
+    return ddx, dPi / np.outer(sd, sd), dxk, dPk, dict(L=L, zero=zero, ratio=ratio)
+
+
+def slam_bounds(P, cols, X, G, ref, tol=GRAM_TOL):
+    """(dx bound, P+ bound Jacobi-scaled by P, factor info) of the library's update against slam_update_reference(P, cols, X): G the
+    library's Gram matrix (nc1 x nc1, lower triangle read), ref the reference.  The factor info: dict(L, zero, ratio)."""
+    nc = len(cols)
+    ddx, dPi, dxk, dPk, fac = gram_route_bounds(P, cols, G, ref, tol, dG=gram_bound(X))
+    dxb, dPb, _ = kalman_bounds(P, list(cols), X[:, :nc], ref)
+    return np.maximum(dxb, dxk) + ddx, np.maximum(dPb, dPk) + dPi, fac
 
 
 # ---- StateHelper::marginalize_slam ---------------------------------------------------------------------------------------------------
