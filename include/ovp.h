@@ -392,6 +392,58 @@ typedef struct ovp_triangulation_mode {
 } ovp_triangulation_mode;
 int ovp_set_triangulation_mode(ovp_ctx *ctx, const ovp_triangulation_mode *m);
 
+/* ---- TrackPlane::perform_plane_detection_monocular (track_plane/TrackPlane.cpp:580-1121): plane detection among tracked features -------
+ * One mono tracker per context, kept on the device across calls like TrackPlane's hist_* members: per feature the bearing system A, b and
+ * its observation count, the triangulated position hist_feat_inG and the window of triangle normals; the feature -> plane map, the merge
+ * history and the plane id counter (starts at 1, never reset).  Each frame triangulates the features with enough observations, builds the
+ * Delaunay mesh of the survivors' pixels (CDT's incremental insertion in the order given, super-triangle erased), pushes each triangle's
+ * normal into its vertices' windows, matches and merges features into planes serially in ascending id, spatially filters every plane with
+ * more than filter_num_feat active features (k-NN z-test) and prunes to the frame's planes with more than 3 active features. */
+#define OVP_PLANE_TRACK_MAX_POINTS 2048    /* features per frame: one CTA holds the frame's mesh in shared memory */
+#define OVP_PLANE_TRACK_MAX_NORM_COUNT 16  /* max_norm_count: normals kept per feature */
+#define OVP_PLANE_TRACK_MAX_FILTER_FEAT 32 /* filter_num_feat: neighbours of the spatial filter's k-NN */
+#define OVP_PLANE_TRACK_MAX_MERGES 16384   /* (plane, old plane) pairs of the merge history */
+typedef struct ovp_plane_track_options { /* TrackPlaneOptions (track_plane/TrackPlaneOptions.h:41-80); defaults in brackets */
+  int max_tri_side_px;       /* [200] a triangle with a longer side (pixels) gives no normal */
+  int max_norm_count;        /* [5] normals kept per feature, 1..OVP_PLANE_TRACK_MAX_NORM_COUNT */
+  double max_norm_avg_max;   /* [25] deg, largest deviation from a feature's average normal */
+  double max_norm_avg_var;   /* [25] deg, standard deviation of the deviations */
+  double max_norm_deg;       /* [25] deg, angle between two matched features' normals */
+  double max_dist_between_z; /* [0.10] m, point-to-plane distance of a match */
+  int max_pairwise_px;       /* [100] pixel distance of a match */
+  int min_norms;             /* [3] normals a feature needs before it matches */
+  int check_old_feats;       /* [1] match features that already have a plane (0 / 1) */
+  int filter_num_feat;       /* [4] k of the spatial filter, 2..OVP_PLANE_TRACK_MAX_FILTER_FEAT */
+  double filter_z_thresh;    /* [1.2] z-test threshold of the spatial filter */
+  int feat_init_min_obs;     /* [4] observations before a feature is triangulated */
+  double min_dist;           /* [0.10] m, depth range of a triangulated feature */
+  double max_dist;           /* [60] */
+  double max_cond_number;    /* [8000] condition number of the bearing system */
+} ovp_plane_track_options;
+/* The tracker's options (NULL: the defaults above).  Accepted only before the first frame (TrackPlane takes its options at construction),
+ * afterwards OVP_ERR_BAD_ARGS.  Out of range (max_norm_count or filter_num_feat outside the ranges above, check_old_feats not 0 / 1,
+ * feat_init_min_obs < 1, a NaN threshold) is OVP_ERR_BAD_ARGS with the options held before kept.  Host-only. */
+int ovp_plane_track_set_options(ovp_ctx *ctx, const ovp_plane_track_options *opt);
+/* One call of perform_plane_detection_monocular on the frame's tracked features, in the tracker's order (CDT's insertion order).
+ * pose_GtoI7 / calib7: hist_state.at(time) / hist_calib.at(cam) as [q_GtoI / q_ItoC (JPL, xyzw), p_IinG / p_IinC].  featid[n]; uv[2n] the
+ * raw pixels, uv_norm[2n] undistort_cv of them.  n == 0 is a no-op.  Refused with OVP_ERR_BAD_ARGS, the tracker untouched and nothing
+ * launched: options never set, a null pointer, a negative featid, a duplicate featid, a non-finite pixel, two features on the same pixel
+ * (CDT keeps a degenerate mesh there), n above OVP_PLANE_TRACK_MAX_POINTS.  The frame crosses to the device in one copy; nothing comes back. */
+int ovp_plane_track_frame(ovp_ctx *ctx, const double pose_GtoI7[7], const double calib7[7], int n, const int64_t *featid, const float *uv,
+                          const float *uv_norm);
+/* hist_feat_to_plane (get_feature2plane) after the last frame, ascending featid; *n entries (cap: the arrays' length, too short:
+ * OVP_ERR_CAPACITY with *n set).  OVP_ERR_CAPACITY also when the merge history outgrew OVP_PLANE_TRACK_MAX_MERGES. */
+int ovp_plane_track_feature2plane(ovp_ctx *ctx, int cap, int64_t *featid, int64_t *planeid, int *n);
+/* hist_plane_to_oldplanes (get_plane2oldplane) as (plane, old plane) pairs sorted by plane then old plane; *n pairs */
+int ovp_plane_track_plane2oldplane(ovp_ctx *ctx, int cap, int64_t *planeid, int64_t *oldplaneid, int *n);
+/* The last frame's mesh (tri_cdt_tri / tri_cdt_tri_norms): tri3[3 * n_tri] index the frame's surviving (triangulated) features in the
+ * order they were given, normal3[3 * n_tri] the normal in G, zero for a triangle rejected by max_tri_side_px.  Either array may be NULL. */
+int ovp_plane_track_mesh(ovp_ctx *ctx, int cap, int *tri3, double *normal3, int *n_tri);
+/* The mesh's vertices after the last frame (tri_cdt_vert_ids / tri_cdt_verts / tri_cdt_vert_pts): the features that had a 3D estimate, in the
+ * order the frame gave them; featid[*n] and their pixels uv[2 * *n].  tri3 of ovp_plane_track_mesh indexes these.  Too short: OVP_ERR_CAPACITY
+ * with *n set. */
+int ovp_plane_track_vertices(ovp_ctx *ctx, int cap, int64_t *featid, float *uv, int *n);
+
 /* ---- PlaneFitting (track_plane/PlaneFitting.cpp): plane hypothesis + refinement, the step right before the plane Jacobians ----------- */
 /* Call sites: UpdaterMSCKF.cpp:267-360, UpdaterPlane.cpp:230-267, UpdaterSLAM.cpp:171.  Both entry points take a BATCH of candidate planes
  * (feat_offset: n_planes + 1 prefix offsets into the per-feature arrays, starting at 0 and never decreasing, else OVP_ERR_BAD_ARGS) and run

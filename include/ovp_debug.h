@@ -114,6 +114,10 @@ int ovp_debug_slam_update(ovp_ctx *ctx, int F, const int *meas_offset, const int
 int ovp_debug_slam_gram(ovp_ctx *ctx, int F, const int *meas_offset, const int *meas_clone, const float *uv, const int64_t *featid,
                         const int64_t *planeid, const ovp_updater_options *opt, int use_plane_constraint, int gcap, double *G_out, int *info,
                         int *cols_out, int *feat_status, double *feat_chi2, double *raw_out);
+/* the plane tracker's history of each feature of featid[n] (tests/test_gpu_plane_track.py), per feature: A (9, row-major), b (3), count
+ * (as a double), has_inG (0 / 1), hist_feat_inG (3), the window length, then OVP_PLANE_TRACK_MAX_NORM_COUNT normals (3 each, oldest first,
+ * zero past the length): 18 + 3 * OVP_PLANE_TRACK_MAX_NORM_COUNT doubles.  A feature the tracker does not hold reads as all zeros. */
+int ovp_debug_plane_track_history(ovp_ctx *ctx, int n, const int64_t *featid, double *out);
 
 #ifdef __cplusplus
 }

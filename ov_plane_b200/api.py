@@ -78,6 +78,20 @@ def _tri_options(options):
     return TriangulationOptions(**{k: (int if t is C.c_int else float)(options[k]) for k, t in TriangulationOptions._fields_})
 
 
+class PlaneTrackOptions(C.Structure):
+    """ovp_plane_track_options: TrackPlaneOptions (include/ovp.h)"""
+    _fields_ = [("max_tri_side_px", C.c_int), ("max_norm_count", C.c_int), ("max_norm_avg_max", C.c_double), ("max_norm_avg_var", C.c_double),
+                ("max_norm_deg", C.c_double), ("max_dist_between_z", C.c_double), ("max_pairwise_px", C.c_int), ("min_norms", C.c_int),
+                ("check_old_feats", C.c_int), ("filter_num_feat", C.c_int), ("filter_z_thresh", C.c_double), ("feat_init_min_obs", C.c_int),
+                ("min_dist", C.c_double), ("max_dist", C.c_double), ("max_cond_number", C.c_double)]
+
+
+PLANE_TRACK_DEFAULTS = dict(max_tri_side_px=200, max_norm_count=5, max_norm_avg_max=25.0, max_norm_avg_var=25.0, max_norm_deg=25.0,
+                            max_dist_between_z=0.10, max_pairwise_px=100, min_norms=3, check_old_feats=1, filter_num_feat=4, filter_z_thresh=1.2,
+                            feat_init_min_obs=4, min_dist=0.10, max_dist=60.0, max_cond_number=8000.0)
+PLANE_TRACK_MAX_POINTS, PLANE_TRACK_MAX_NORM_COUNT = 2048, 16
+
+
 class PlaneInitOptions(C.Structure):
     _fields_ = [("sigma_pix", C.c_double), ("max_msckf_plane", C.c_int), ("plane_init_min_feat", C.c_int), ("plane_init_max_cond", C.c_double),
                 ("shuffle_kind", C.c_int), ("tri", C.c_void_p)]
@@ -625,6 +639,74 @@ class Context(object):
             return
         m = TriangulationMode(int(triangulate_1d), int(refine_features))
         self._ck(self.lib.ovp_set_triangulation_mode(self.h, C.byref(m)))
+
+    # ---- TrackPlane::perform_plane_detection_monocular (the front end's plane detection) ----
+    def plane_track_set_options(self, options=None):
+        """options: a dict of PlaneTrackOptions fields (missing ones take the defaults), None: the defaults.  Before the first frame only."""
+        if options is None:
+            self._ck(self.lib.ovp_plane_track_set_options(self.h, None))
+            return
+        o = dict(PLANE_TRACK_DEFAULTS, **options)
+        opt = PlaneTrackOptions(**{k: (int if t is C.c_int else float)(o[k]) for k, t in PlaneTrackOptions._fields_})
+        self._ck(self.lib.ovp_plane_track_set_options(self.h, C.byref(opt)))
+
+    def plane_track_frame(self, pose_GtoI7, calib7, featid, uv, uv_norm):
+        """one frame: pose / calib as [q (JPL xyzw), p], featid (n,), uv / uv_norm (n, 2) float32 in the tracker's order"""
+        q, cb = _f64(pose_GtoI7), _f64(calib7)
+        fid = np.ascontiguousarray(featid, dtype=np.int64)
+        u = np.ascontiguousarray(uv, dtype=np.float32).reshape(-1, 2)
+        un = np.ascontiguousarray(uv_norm, dtype=np.float32).reshape(-1, 2)
+        if len(u) != len(fid) or len(un) != len(fid):
+            raise ValueError("featid, uv and uv_norm differ in length")
+        self._ck(self.lib.ovp_plane_track_frame(self.h, _p(q), _p(cb), len(fid), _p(fid), _p(u), _p(un)))
+
+    def plane_track_feature2plane(self):
+        """{featid: planeid} (get_feature2plane)"""
+        n = C.c_int(0)
+        cap = PLANE_TRACK_MAX_POINTS
+        f, p = np.zeros(cap, dtype=np.int64), np.zeros(cap, dtype=np.int64)
+        self._ck(self.lib.ovp_plane_track_feature2plane(self.h, cap, _p(f), _p(p), C.byref(n)))
+        return {int(a): int(b) for a, b in zip(f[:n.value], p[:n.value])}
+
+    def plane_track_plane2oldplane(self):
+        """{planeid: set of old plane ids} (get_plane2oldplane)"""
+        n = C.c_int(0)
+        cap = 16384  # OVP_PLANE_TRACK_MAX_MERGES
+        p, o = np.zeros(cap, dtype=np.int64), np.zeros(cap, dtype=np.int64)
+        self._ck(self.lib.ovp_plane_track_plane2oldplane(self.h, cap, _p(p), _p(o), C.byref(n)))
+        out = {}
+        for a, b in zip(p[:n.value], o[:n.value]):
+            out.setdefault(int(a), set()).add(int(b))
+        return out
+
+    def plane_track_mesh(self):
+        """(tri (T, 3) int32 indices of the frame's triangulated features in order, normals (T, 3), zero for a rejected triangle)"""
+        n = C.c_int(0)
+        self._ck(self.lib.ovp_plane_track_mesh(self.h, 0, None, None, C.byref(n)))
+        T = n.value
+        tri, nrm = np.zeros((max(T, 1), 3), dtype=np.int32), np.zeros((max(T, 1), 3))
+        self._ck(self.lib.ovp_plane_track_mesh(self.h, T, _p(tri), _p(nrm), C.byref(n)))
+        return tri[:T], nrm[:T]
+
+    def plane_track_vertices(self):
+        """(featid (m,), uv (m, 2) float32): the features the last frame's mesh indexes, in the frame's order"""
+        n = C.c_int(0)
+        cap = PLANE_TRACK_MAX_POINTS
+        f, u = np.zeros(cap, dtype=np.int64), np.zeros((cap, 2), dtype=np.float32)
+        self._ck(self.lib.ovp_plane_track_vertices(self.h, cap, _p(f), _p(u), C.byref(n)))
+        return f[:n.value].copy(), u[:n.value].copy()
+
+    def plane_track_history(self, featid):
+        """debug library only: per feature (A 3x3, b, count, has_inG, p_FinG, window (len, 3)) of the tracker's history"""
+        fid = np.ascontiguousarray(featid, dtype=np.int64)
+        rec = 18 + 3 * PLANE_TRACK_MAX_NORM_COUNT
+        out = np.zeros((max(len(fid), 1), rec))
+        self._ck(self.lib.ovp_debug_plane_track_history(self.h, len(fid), _p(fid), _p(out)))
+        res = []
+        for r in out[:len(fid)]:
+            wl = int(r[17])
+            res.append(dict(A=r[:9].reshape(3, 3), b=r[9:12], count=int(r[12]), has=bool(r[13]), p_FinG=r[14:17], window=r[18:18 + 3 * wl].reshape(wl, 3)))
+        return res
 
     # ---- PlaneFitting (plane hypothesis + refinement, the step before the plane Jacobians) ----
     def plane_fitting(self, feat_offset, p_FinG, min_inlier_num, max_cond, shuffle_kind=0):

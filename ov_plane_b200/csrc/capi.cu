@@ -495,6 +495,7 @@ void ovp_destroy(ovp_ctx *h) {
   cudaFree(c->d_chi2_table);
   cudaFree(c->d_batch);
   cudaFree(c->d_stage);
+  plane_track_free(c);
   cudaFree(c->snapP);
   cudaFree(c->snap_val);
   cudaFree(c->snap_fej);

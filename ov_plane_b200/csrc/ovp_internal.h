@@ -37,6 +37,7 @@ struct DenseWs {
 };
 
 struct Prepared; // the plan of the last prepared MSCKF batch (features_host.inc)
+struct PlaneTrack; // the mono plane tracker (plane_track.cu)
 
 struct Ctx {
   int device = 0;
@@ -181,6 +182,7 @@ struct Ctx {
   cudaEvent_t prof_pending = nullptr;
   int prof_pending_id = 0;
   double prof_pending_work = 0;
+  PlaneTrack *ptrack = nullptr; // created by the first ovp_plane_track_* call
 };
 enum { PROF_GEMM = 0, PROF_GRAM = 1, PROF_POTRF = 2, PROF_FEATURE = 3, PROF_OTHER = 4, PROF_N = 5 };
 void prof_begin(Ctx *c, int id, double work);
@@ -189,6 +191,7 @@ int msckf_prepare(Ctx *c, const ovp_feature_batch *b, const ovp_updater_options 
 int msckf_launch(Ctx *c);
 int msckf_finish(Ctx *c, int *feat_status, double *feat_chi2, int *plane_status, double *plane_chi2, int *hx_order, int *hx_order_n);
 void free_prepared(Ctx *c);
+void plane_track_free(Ctx *c);
 void drop_prepared_graph(Ctx *c); // the prepared batch's captured graph: its next launch captures the plan again
 
 // error helpers

@@ -8,6 +8,7 @@
 #include "capi2.cu"
 #include "planefit.cu"
 #include "anchors.cu"
+#include "plane_track.cu"
 #ifdef OVP_DEBUG // libovp_debug.so only: micro-benchmarks and kernel-level test hooks (include/ovp_debug.h)
 #include "debug_hooks.cu"
 #endif
